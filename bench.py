@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""SwapNet GAN-training throughput on B200 (BASELINE.json metric: images/s of the full G+D training step).
+"""SwapNet GAN-training throughput on H100 (BASELINE.json metric: images/s of the full G+D training step).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (default: warp stage, configs[1])
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (baseline arm, same config object)
@@ -7,6 +7,7 @@
     python bench.py --model texture --perceptual             # BASELINE configs[2] (default texture losses incl. VGG16)
     python bench.py --model joint --perceptual               # configs[4]: one warp + one texture step, 8 images/GPU
     python bench.py --device-augment                         # e2e leg with the dataset's augmentation on the device (f4)
+    python bench.py --dump-outputs DIR                       # also write what the last timed step computed to DIR/*.npy
 
 One "step" = one `optimize_parameters()` of the plugin (G fwd, D step on fake+real, G step through D, both AdamW updates —
 the full reference training step, models/warp_model.py:169-183 / texture_model.py:127-180) on a synthetic batch of
@@ -19,12 +20,17 @@ libraries print (NCCL banner ...) is routed to stderr.  Field notes:
             tensors travel as uint8 label maps (ops.SegMap, expanded on the device) unless --fp32-inputs (the 19-channel
             fp32 tensors the reference's DataLoader yields: 688 MB per batch-16 step); --device-augment ships one label
             map per sample + the drawn op table and runs the per-channel augmentation on the device inside the region;
-  roofline  dominant kernel class = the tcgen05 tap-GEMM (`tap_gemm_kernel<3>`: forward + dgrad launches): algorithmic
-            conv FLOPs of those launches / their summed CUDA-event time in one extra eager step, against the measured
-            sustained dense bf16 peak (MEASURED_PEAKS.json).  The kernel issues 3 MMAs per algorithmic MAC (fp16/bf16-split
+  roofline  dominant kernel class = the wgmma tap-GEMM (`tap_gemm_kernel<3,...>`: forward + dgrad launches): algorithmic
+            conv FLOPs of those launches / their summed CUDA-event time in one extra eager step, against the dense bf16
+            peak (MEASURED_PEAKS.json if present, else the H100 SXM data sheet's 989 TFLOP/s at 700 W, which a card at a
+            lower power limit does not reach).  The kernel issues 3 MMAs per algorithmic MAC (fp16/bf16-split
             fp32-faithful product), so frac <= 1/3 by construction; `pipe_frac` is the tensor-pipe view (3x);
             `resblock` = the eight resblock convs alone (fwd / dgrad / wgrad), `wgrad_kernel` = all weight gradients;
-            `traffic` = DRAM bytes per launch from the committed ncu capture (a constant from profiles/, not measured here);
+  gpu       name and power limit of the card the numbers were measured on (nvidia-smi, read in the same run);
+  --dump-outputs DIR  after the timed steps: per stage, what the last timed step handed to its caller — the generator
+            output `fakes`, the losses, and the updated generator weights — as DIR/<stage>_<name>.npy (float32; losses
+            float64).  Arrays larger than DUMP_SAMPLE elements are a fixed seeded sample of their flat indices, the same
+            from run to run, as are the inputs: two builds compare output for output;
   cpu_baseline  the CPU oracle port (oracle/nets.py, pinned bit-exactly to the reference modules) running the same
             training step at 512x512, batch 1, on the host cores the cgroup quota allows (host_cores()), `--cpu-steps`
             steps (N = 1 only; --no-cpu-baseline skips it);
@@ -164,7 +170,7 @@ def warp_opt(B, S, precision):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -197,14 +203,42 @@ class ClockSampler(threading.Thread):
                 "samples": len(self.rows)}
 
 
-def ncu_traffic():
-    """dram__bytes_read + dram__bytes_write per launch of the dominant kernel, from the committed
-    `ncu --set full` capture (profiles/r02_ncu_traffic.json); null if absent."""
-    for name in ("r02_ncu_traffic.json", "r01_ncu_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            return json.load(open(p))
-    return None
+def gpu_info(index: int):
+    """Name and power limit (W) of the card: a measured number is only meaningful with both beside it."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout
+        name, limit = [x.strip() for x in out.strip().split(",")][:2]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+
+
+DUMP_SAMPLE = 1 << 22       # elements kept of a larger array by --dump-outputs (16 MB in float32)
+
+
+def dump_outputs(legs, out_dir):
+    """--dump-outputs: write, per stage, what the last `optimize_parameters()` handed to its caller (see the module doc)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+
+    def sample(t, n):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > n:
+            idx = torch.randint(0, flat.numel(), (n,), generator=torch.Generator().manual_seed(0)).sort().values
+            flat = flat[idx.to(flat.device)]
+        return flat.float().cpu().numpy()
+
+    for m, *_ in legs:
+        stage = m.opt.model
+        fakes = m.fakes.detach()
+        arr = fakes.float().cpu().numpy() if fakes.numel() <= DUMP_SAMPLE else sample(fakes, DUMP_SAMPLE)
+        np.save(os.path.join(out_dir, f"{stage}_fakes.npy"), arr)
+        losses = m.get_current_losses()
+        np.save(os.path.join(out_dir, f"{stage}_losses.npy"), np.array(list(losses.values()), dtype=np.float64))
+        weights = torch.cat([p.detach().reshape(-1) for p in m.net_generator.parameters()])
+        np.save(os.path.join(out_dir, f"{stage}_generator_weights.npy"), sample(weights, DUMP_SAMPLE // 4))
 
 
 def measured_peaks():
@@ -212,7 +246,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, 700 W; not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -415,6 +449,8 @@ def main():
     ap.add_argument("--cpu-steps", type=int, default=3,
                     help="timed CPU-oracle steps of the cpu_baseline leg (one step = ~5 s on the usable host cores)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<stage>_<name>.npy")
     ap.add_argument("--perceptual", action="store_true",
                     help="--model texture: add the VGG16 content + Gram style terms (lambda 20 / 1e-8)")
     ap.add_argument("--model", default="warp", choices=("warp", "texture", "joint"),
@@ -435,7 +471,7 @@ def main():
         "joint": f"joint warp+texture {S}x{S} synthetic, batch {B}/GPU, one full warp GAN step + one full texture GAN step "
                  f"per iteration ({tex_losses})"}[args.model]
     config = {"workload": workload, "global_batch": B * world, "parallelism": f"dp{world}",
-              "l2": "inputs+activations per step (>2 GB) exceed the 126 MB L2; no explicit flush",
+              "l2": "inputs+activations per step (>2 GB) exceed the 50 MB L2; no explicit flush",
               "algorithmic_tflop_per_step": step_gflop_per_img(args) * (S / 512) ** 2 * B * world / 1e3}
 
     if args.impl == "reference":
@@ -552,6 +588,8 @@ def main():
     ms = timed(args.steps, False, False)
     launches = ops.launch_count() - l0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(legs, args.dump_outputs)
     for _ in range(2):                      # the host-input path has its own staging buffers: warm them
         one_step(True, True)
     ms_e2e = timed(args.steps, True, True)
@@ -602,16 +640,11 @@ def main():
         res_fl = tot["res_fwd"][0] + tot["res_dgrad"][0]
         res_ms = tot["res_fwd"][1] + tot["res_dgrad"][1]
         res = (res_fl / (res_ms * 1e-3) / 1e12) if res_ms else 0.0
-        tr = ncu_traffic()
-        roof = {"bound": "tensor", "kernel": "tap_gemm_kernel<3> (tcgen05, fwd+dgrad launches)", "achieved": ach,
+        roof = {"bound": "tensor", "kernel": "tap_gemm_kernel<3,...> (wgmma, fwd+dgrad launches)", "achieved": ach,
                 "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "pipe_frac": 3 * ach / peak, "peak_source": how,
                 "launches_per_step": gemm_n, "avg_launch_ms": gemm_ms / max(gemm_n, 1),
                 "algorithmic_gflop_per_launch": gemm_fl / max(gemm_n, 1) / 1e9,
                 "share_of_step": gemm_ms / step_ms,
-                # DRAM bytes of one launch of the dominant shape: a constant from the committed `ncu --set full`
-                # capture (profiles/), NOT measured in this run
-                "traffic": (tr or {}).get("dram_bytes_per_launch"), "traffic_source": "committed ncu capture (profiles/)",
-                "traffic_detail": tr,
                 # the fused U-Net conv blocks the north-star target is read against: the 8 resblock convs
                 # (59 % of generator FLOPs), FLOP-weighted over their fwd + dgrad launches, and their wgrad launches
                 "resblock": {"achieved": res, "frac": res / peak, "pipe_frac": 3 * res / peak,
@@ -646,6 +679,7 @@ def main():
                            "on the device inside the timed region (swapnet_b200/data.py)") if args.device_augment else
                 "uint8 label maps for the cloth tensors (ops.SegMap), expanded to one-hot planes on the device"
                 if args.labels else "fp32 tensors as the reference's DataLoader yields them"},
+        "gpu": gpu_info(local), "peak_memory_gb": torch.cuda.max_memory_allocated() / 1e9,
         "gpu_launches": launches, "clocks": clocks, "roofline": roof, "cpu_baseline": cpu,
     }
     if args.device_augment:

@@ -21,7 +21,7 @@
  *     wider concat buffer;
  *   - a GEMM operand is a "split plane pair": two 16-bit-float NHWC tensors hi = r16(v),
  *     lo = r16(v - hi) in format SN_FMT_F16 or SN_FMT_BF16 (fp32 carried as 2 x 16 bit; products are
- *     evaluated as hi*hi + lo*hi + hi*lo on the tcgen05 tensor cores with fp32 accumulation).
+ *     evaluated as hi*hi + lo*hi + hi*lo on the tensor cores (sm_90a wgmma) with fp32 accumulation).
  *     Both operands of one contraction must use the same format: forward GEMMs run fp16-split
  *     (activations x scaled weights), backward GEMMs bf16-split (gradients x bf16 copies).
  */
@@ -230,7 +230,7 @@ typedef struct sn_norm_act_desc {
   int out_fmt;
   void* out2_hi; void* out2_lo; int out2_fmt; /* optional companion planes, same geometry (the
                                             bf16-split copy read by the weight-gradient GEMM: A and B
-                                            of one tcgen05.mma must share a format) */
+                                            of one wgmma must share a format) */
   int out_reflect_pad;                   /* 1: planes are [n, h+2, w+2] with ReflectionPad2d(1) */
   float* out_f32; int f32_pitch;         /* optional fp32 copy (residual stream) */
 } sn_norm_act_desc;
@@ -421,7 +421,7 @@ int sn_augment_channels(const void* labels_u8, const float* dense_nchw, int n, i
 
 /* ------------------------------------------------------------------------------------------
  * reference-free fp32 CUDA-core contraction with the tap-GEMM semantics (no tensor cores).
- * Used by the tests as an on-device cross-check of the tcgen05 path, never by the plugin.
+ * Used by the tests as an on-device cross-check of the wgmma path, never by the plugin.
  * ---------------------------------------------------------------------------------------- */
 int sn_tap_gemm_simt(const sn_tap_gemm_desc* desc, void* stream);
 

@@ -1,4 +1,4 @@
-"""In-tree build of libswapnet_b200.so (sm_100a) with plain nvcc.
+"""In-tree build of libswapnet_b200.so (sm_90a, H100) with plain nvcc.
 
 The library is a C-ABI shared object (include/swapnet_b200.h); nothing here links against
 torch.  Object files live under swapnet_b200/csrc/build/, the .so next to this file so that it
@@ -11,13 +11,14 @@ import os
 import shutil
 import subprocess
 import sys
+from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libswapnet_b200.so")
 SOURCES = ["api.cu", "gemm_tc.cu", "elementwise.cu", "roi_align.cu", "perceptual.cu", "patch_logits.cu", "augment.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -49,14 +50,15 @@ def build(force: bool = False, verbose: bool = True) -> str:
         return OUT
     nvcc = _nvcc()
     os.makedirs(os.path.join(CSRC, "build"), exist_ok=True)
-    objs = []
-    for src in SOURCES:
-        obj = os.path.join(CSRC, "build", src.replace(".cu", ".o"))
-        cmd = [nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
-        if verbose:
+    objs = [os.path.join(CSRC, "build", src.replace(".cu", ".o")) for src in SOURCES]
+    cmds = [[nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj] for src, obj in zip(SOURCES, objs)]
+    if verbose:
+        for cmd in cmds:
             print("[swapnet_b200.build]", " ".join(cmd), file=sys.stderr)
-        subprocess.run(cmd, check=True)
-        objs.append(obj)
+    # the sources are independent translation units: compile them side by side
+    with ThreadPoolExecutor(max_workers=min(len(cmds), os.cpu_count() or 1)) as pool:
+        for _ in pool.map(lambda cmd: subprocess.run(cmd, check=True), cmds):
+            pass
     cmd = [nvcc, "-shared", "-o", OUT, *objs, "-Wno-deprecated-gpu-targets"]
     if verbose:
         print("[swapnet_b200.build]", " ".join(cmd), file=sys.stderr)

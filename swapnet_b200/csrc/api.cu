@@ -27,14 +27,14 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sm_count <= 0) g_sm_count = 148;
+    if (g_sm_count <= 0) g_sm_count = SN_NUM_SMS;
   }
   return g_sm_count;
 }
 
 extern "C" {
 
-const char* sn_version(void) { return "swapnet_b200 0.1.0 (sm_100a, tcgen05 split-bf16)"; }
+const char* sn_version(void) { return "swapnet_b200 0.1.0 (sm_90a, wgmma split-bf16)"; }
 const char* sn_last_error(void) { return g_err; }
 long long sn_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 void sn_count_replayed(long long n) { g_launches.fetch_add(n, std::memory_order_relaxed); }

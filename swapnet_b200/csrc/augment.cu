@@ -1,4 +1,4 @@
-// swapnet_b200 — per-channel cloth augmentation on the device (sm_100a, HBM bound; SURVEY §8 f4).
+// swapnet_b200 — per-channel cloth augmentation on the device (sm_90a, HBM bound; SURVEY §8 f4).
 //
 // Replaces datasets/data_utils.py:346-361 `per_channel_transform` (19 PIL mode-"F" images per sample, each through
 // torchvision's RandomOrder([RandomVerticalFlip, RandomHorizontalFlip, RandomAffine, RandomPerspective]) of

@@ -1,4 +1,4 @@
-// swapnet_b200 — HBM-bound kernels of the SwapNet hot path (sm_100a).
+// swapnet_b200 — HBM-bound kernels of the SwapNet hot path (sm_90a).
 //
 // Operand packing (fp32 -> split-bf16 NHWC planes), InstanceNorm statistics, the fused
 // InstanceNorm-apply + activation + dropout (+ residual, + reflect padding) forward and
@@ -1757,7 +1757,7 @@ inline bool srcs_vec_ok(const GradSrcs& g) {
   return true;
 }
 inline int vslabs(int hw, int n) {  // ~6 waves of 256-thread blocks, at least 32 pixels per block
-  int want = (148 * 6 + n - 1) / n;
+  int want = (SN_NUM_SMS * 6 + n - 1) / n;
   int maxs = (hw + 31) / 32;
   if (want > maxs) want = maxs;
   return want < 1 ? 1 : want;
@@ -1765,7 +1765,7 @@ inline int vslabs(int hw, int n) {  // ~6 waves of 256-thread blocks, at least 3
 
 inline int grid_for(long long total, int threads = kEwThreads) {
   long long g = (total + threads - 1) / threads;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > SN_NUM_SMS * 16) g = SN_NUM_SMS * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -1777,7 +1777,7 @@ inline dim3 cblock(int C) {
 }
 inline int slabs_for(int hw, int n, int py) {
   // enough blocks for ~4 waves, at least `py` pixels each
-  int want = (148 * 4 + n - 1) / n;
+  int want = (SN_NUM_SMS * 4 + n - 1) / n;
   int maxs = (hw + py - 1) / py;
   if (want > maxs) want = maxs;
   if (want < 1) want = 1;
@@ -1937,7 +1937,7 @@ int sn_plane_stats(const float* y, int pitch, int n, int hw, int c, float eps, d
   cudaStream_t st = (cudaStream_t)stream;
   SN_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * c, st));
   const int cg = (c + 31) / 32;
-  int slabs = (148 * 4 + n * cg - 1) / (n * cg);
+  int slabs = (SN_NUM_SMS * 4 + n * cg - 1) / (n * cg);
   if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
   if (slabs < 1) slabs = 1;
   plane_stats_kernel<<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats);
@@ -2038,7 +2038,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       int bx = 1;
       while (bx < d->c / 4 && bx < 32) bx <<= 1;
       const int qg = (d->c / 4 + bx - 1) / bx;
-      int slabs = (148 * 6 + d->n * qg - 1) / (d->n * qg);
+      int slabs = (SN_NUM_SMS * 6 + d->n * qg - 1) / (d->n * qg);
       if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
       if (slabs < 1) slabs = 1;
       if (ew_use_v4()) {
@@ -2050,7 +2050,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       else norm_act_bwd_reduce_v4u_kernel<2><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
     } else {
       const int cg = (d->c + 31) / 32;
-      int slabs = (148 * 4 + d->n * cg - 1) / (d->n * cg);
+      int slabs = (SN_NUM_SMS * 4 + d->n * cg - 1) / (d->n * cg);
       if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
       if (slabs < 1) slabs = 1;
       norm_act_bwd_reduce_kernel<<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
@@ -2088,7 +2088,7 @@ int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int 
   cudaStream_t st = (cudaStream_t)stream;
   SN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * c, st));
   const int cg = (c + 31) / 32;
-  long long slabs = (148 * 4 + cg - 1) / cg;
+  long long slabs = (SN_NUM_SMS * 4 + cg - 1) / cg;
   if (slabs > (npix + 63) / 64) slabs = (npix + 63) / 64;
   if (slabs < 1) slabs = 1;
   const uint16_t* hi = (const uint16_t*)dy_hi + coff;
@@ -2100,7 +2100,7 @@ int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int 
     int bx = 1;
     while (bx < groups && bx < 32) bx <<= 1;
     const int gx = (groups + bx - 1) / bx;
-    long long sl = (148 * 6 + gx - 1) / gx;
+    long long sl = (SN_NUM_SMS * 6 + gx - 1) / gx;
     if (sl > (npix + 255) / 256) sl = (npix + 255) / 256;
     if (sl < 1) sl = 1;
     bias_grad_v8_kernel<<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch);

@@ -1,4 +1,4 @@
-// swapnet_b200 — tcgen05 implicit-GEMM kernels (sm_100a).
+// swapnet_b200 — wgmma implicit-GEMM kernels (sm_90a).
 //
 // Every dense contraction of the SwapNet hot path (reference call sites:
 // modules/layers.py:15,31,131-138  Conv2d 4x4 s2 / ConvTranspose2d 4x4 s2 /
@@ -19,13 +19,14 @@
 //     G[i, j] (+)= sum_{pixels (n,h,w)} X[n, h + dh, w + dw, i] * Y[n, h + dh', w + dw', j]
 //   both operands are activation patches; the reduction runs over pixels.
 //
-// Arithmetic: bf16 tensor-core MMAs (tcgen05.mma kind::f16) with fp32
-// accumulation in TMEM.  NSPLIT = 3 evaluates hi*hi + lo*hi + hi*lo, i.e. an
+// Arithmetic: 16-bit tensor-core MMAs (wgmma.mma_async, bf16 or f16) with fp32
+// accumulation in registers.  NSPLIT = 3 evaluates hi*hi + lo*hi + hi*lo, i.e. an
 // fp32-faithful product (~2^-16 relative) as the 1e-3 fp32 parity bar requires;
 // NSPLIT = 1 is the single-pass bf16 fast mode.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA
-// issuer, warps 2..5 = epilogue (TMEM -> registers -> global).
+// Warp roles (288 threads): warps 0..7 = two MMA warpgroups (64 rows of the
+// 128-row tile each; they also run the epilogue, registers -> global), warp 8 =
+// TMA producer.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -36,7 +37,9 @@ namespace {
 constexpr int kBlockM = 128;
 constexpr int kTileRing = 4;
 constexpr int kTileBytes = 16384;  // 128 rows x 128 B (one operand plane of one stage)
-constexpr int kThreads = 192;
+constexpr int kConsumerWarps = 8;  // two MMA warpgroups, 64 of the 128 tile rows each
+constexpr int kProducerWarp = kConsumerWarps;
+constexpr int kThreads = (kConsumerWarps + 1) * 32;
 
 template <int NSPLIT>
 struct Cfg {
@@ -51,65 +54,37 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-// Column sums over a warp's 32 rows of a 32 x 16 register tile (x[j] = this lane's value of column j): a butterfly that
-// halves the number of live values at every exchange (8 + 4 + 2 + 1 + 1 = 16 shuffles instead of 16 x 5).  On return
-// x[0] holds the total of column (lane >> 1) — both lanes of a pair hold the same total.
-__device__ __forceinline__ void col_sums16(float (&x)[16], int lane) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const bool up = lane & 16;
-    const float send = up ? x[j] : x[j + 8];
-    const float recv = __shfl_xor_sync(0xffffffffu, send, 16);
-    x[j] = (up ? x[j + 8] : x[j]) + recv;
-  }
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const bool up = lane & 8;
-    const float send = up ? x[j] : x[j + 4];
-    const float recv = __shfl_xor_sync(0xffffffffu, send, 8);
-    x[j] = (up ? x[j + 4] : x[j]) + recv;
-  }
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const bool up = lane & 4;
-    const float send = up ? x[j] : x[j + 2];
-    const float recv = __shfl_xor_sync(0xffffffffu, send, 4);
-    x[j] = (up ? x[j + 2] : x[j]) + recv;
-  }
-  {
-    const bool up = lane & 2;
-    const float send = up ? x[0] : x[1];
-    const float recv = __shfl_xor_sync(0xffffffffu, send, 2);
-    x[0] = (up ? x[1] : x[0]) + recv;
-  }
-  x[0] += __shfl_xor_sync(0xffffffffu, x[0], 1);
+// Sum over the 8 rows held by lanes with the same (lane % 4): after the call every lane holds its column's total over
+// the warp's 16 accumulator rows (given v = the sum of the lane's two rows).
+__device__ __forceinline__ float quad_col_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  v += __shfl_xor_sync(0xffffffffu, v, 16);
+  return v;
 }
 
 // ============================================================================
 // conv mode
 // ============================================================================
-// CW = channels per A row (64 / 32 / 16): a template parameter so that the single MMA-issuing thread
-// carries no runtime index arithmetic (measured: runtime div/mod there costs 30 % of the kernel).
-template <int NSPLIT, int CW>
+// CW = channels per A row (64 / 32 / 16) and BN = MMA N (>= block_n): template parameters so that the MMA loop
+// carries no runtime index arithmetic.  F16: both operands f16 (else bf16).
+template <int NSPLIT, int CW, int BN, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, const int n_tiles, const int total_tiles) {
   // Persistent: one CTA per SM walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... (M tile fastest, then N tile,
-  // then output-parity phase).  The smem ring keeps running across tiles and the accumulator is double
-  // buffered in TMEM (2 x 128 columns), so the epilogue of tile i overlaps the main loop of tile i + 1 and
-  // the pipeline prologue is paid once per CTA instead of once per tile.
+  // then output-parity phase).  The smem ring keeps running across tiles, so the producer loads the next tile's
+  // stages while the MMA warpgroups run the epilogue of the current one, and the pipeline prologue is paid once per
+  // CTA instead of once per tile.
   using C = Cfg<NSPLIT>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[C::kStages];
   __shared__ __align__(8) uint64_t empty_bar[C::kStages];
-  __shared__ __align__(8) uint64_t tfull_bar[2];    // MMA -> epilogue: accumulator b complete
-  __shared__ __align__(8) uint64_t tempty_bar[2];   // epilogue -> MMA: accumulator b drained (4 warps)
   // dynamic tile schedule (p.tile_counter != null): the producer draws tile numbers from a device counter and hands them
-  // to the MMA and epilogue warps through a 4-deep ring, so a CTA that becomes resident late (SMs held by NCCL or by the
+  // to the MMA warps through a 4-deep ring, so a CTA that becomes resident late (SMs held by NCCL or by the
   // weight-gradient stream's CTAs) finds only the tiles nobody has taken yet instead of a fixed 1/gridDim share
   __shared__ __align__(8) uint64_t tr_full[kTileRing];
   __shared__ __align__(8) uint64_t tr_empty[kTileRing];
   __shared__ int tile_ring[kTileRing];
-  __shared__ uint32_t tmem_base_smem;
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -126,31 +101,23 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], 4);
+      mbar_init(&empty_bar[s], 2);    // one arrival per MMA warpgroup
     }
     for (int r = 0; r < kTileRing; ++r) {
       mbar_init(&tr_full[r], 1);
-      mbar_init(&tr_empty[r], 5);     // the MMA thread + the four epilogue warps
+      mbar_init(&tr_empty[r], kConsumerWarps);
     }
     mbar_fence_init();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     for (int pl = 0; pl < C::kPlanes; ++pl) {
       tma_prefetch_desc(&p.tmA[pl]);
       tma_prefetch_desc(&p.tmB[pl]);
     }
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       const uint32_t stage_tx = C::kPlanes * (p.a_rows * 128 + p.block_n * 128);
@@ -225,66 +192,22 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
         tile = next;
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_16(kBlockM, p.block_n, p.a_fmt, p.b_fmt, 0, 0);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x;; tile += gridDim.x, ++tcount) {
-        if (dyn) {
-          const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
-          mbar_wait(&tr_full[slot], rph);
-          tile = tile_ring[slot];
-          mbar_arrive(&tr_empty[slot]);
-          if (tile < 0) break;
-        } else if (tile >= total_tiles) {
-          break;
-        }
-        const uint32_t b = tcount & 1;
-        mbar_wait(&tempty_bar[b], ((tcount >> 1) & 1) ^ 1);   // the epilogue has drained accumulator b
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + b * 128;
-        uint32_t acc = 0;
-        for (int k = 0; k < k_iters; ++k, ++it) {
-          const uint32_t s = it % C::kStages;
-          const uint32_t ph = (it / C::kStages) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t st = smem_base + s * C::kStageBytes;
-          // K-major, rows of cw channels: SWIZZLE_128B/64B/32B, SBO = 8 rows, LBO unused (1)
-          constexpr uint32_t a_layout = cw >= 64 ? 2u : (cw == 32 ? 4u : 6u);
-          constexpr uint32_t a_sbo = 8u * cw * 2u;
-          const uint64_t a_hi = umma_smem_desc(st, 16, a_sbo, a_layout);
-          const uint64_t b_hi = umma_smem_desc(st + C::kPlanes * kTileBytes, 16, 1024);
-          const uint64_t a_lo = umma_smem_desc(st + p.a_lo_off, 16, a_sbo, a_layout);
-          const uint64_t b_lo = umma_smem_desc(st + C::kPlanes * kTileBytes + p.b_lo_off, 16, 1024);
-          constexpr uint32_t sub16 = (uint32_t)(128 * cw * 2) >> 4;  // sub-tile stride in 16-B units
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {  // 4 x (UMMA_K = 16 elements = 32 B) per 64-deep stage
-            const uint64_t badv = (uint64_t)(kk * 2);
-            // A: k-step kk lives in sub-tile (16kk / cw), at byte offset ((16kk) % cw) * 2 of its rows
-            const uint64_t aadv = (uint64_t)(((kk * 16) / cw) * sub16 + (((kk * 16) % cw) >> 3));
-            umma_bf16(tmem_d, a_hi + aadv, b_hi + badv, idesc, acc);
-            acc = 1;
-            if (NSPLIT == 3) {
-              umma_bf16(tmem_d, a_lo + aadv, b_hi + badv, idesc, 1);
-              umma_bf16(tmem_d, a_hi + aadv, b_lo + badv, idesc, 1);
-            }
-          }
-          umma_commit(&empty_bar[s]);  // frees the smem stage once these MMAs retire
-        }
-        umma_commit(&tfull_bar[b]);
-      }
-    }
   } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;  // TMEM lane quadrant this warp may read
-    const int row = q * 32 + lane;
-    const int w_i = row % p.tw;
-    const int h_i = (row / p.tw) % p.th;
-    const int n_i = row / (p.tw * p.th);
+    // ===================== MMA warpgroups + epilogue =====================
+    const int wg = warp >> 2;                              // rows [64 wg, 64 wg + 64) of the tile
+    const int quad = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+    int w_i[2], h_i[2], n_i[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      w_i[h] = row % p.tw;
+      h_i[h] = (row / p.tw) % p.th;
+      n_i[h] = row / (p.tw * p.th);
+    }
     const float oscale = p.b_scale ? p.b_scale[1] : 1.f;  // undo the power-of-two weight scale (exact)
-    uint32_t tcount = 0;
+    float acc[BN / 2];
+    uint32_t it = 0, tcount = 0;
     for (int tile = blockIdx.x;; tile += gridDim.x, ++tcount) {
       if (dyn) {
         const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
@@ -296,100 +219,124 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
       } else if (tile >= total_tiles) {
         break;
       }
+      for (int k = 0; k < k_iters; ++k, ++it) {
+        const uint32_t s = it % C::kStages;
+        const uint32_t ph = (it / C::kStages) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t st = smem_base + s * C::kStageBytes;
+        // K-major, rows of cw channels: SWIZZLE_128B/64B/32B, SBO = 8 rows; this warpgroup's 64 rows start
+        // 64 rows into every A sub-tile
+        constexpr uint32_t a_layout = cw >= 64 ? 1u : (cw == 32 ? 2u : 3u);
+        constexpr uint32_t a_sbo = 8u * cw * 2u;
+        const uint32_t a_row0 = (uint32_t)wg * 64u * cw * 2u;
+        const uint64_t a_hi = gmma_smem_desc(st + a_row0, 16, a_sbo, a_layout);
+        const uint64_t b_hi = gmma_smem_desc(st + C::kPlanes * kTileBytes, 16, 1024);
+        const uint64_t a_lo = gmma_smem_desc(st + p.a_lo_off + a_row0, 16, a_sbo, a_layout);
+        const uint64_t b_lo = gmma_smem_desc(st + C::kPlanes * kTileBytes + p.b_lo_off, 16, 1024);
+        constexpr uint32_t sub16 = (uint32_t)(128 * cw * 2) >> 4;  // sub-tile stride in 16-B units
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {  // 4 x (K = 16 elements = 32 B) per 64-deep stage
+          const uint64_t badv = (uint64_t)(kk * 2);
+          // A: k-step kk lives in sub-tile (16kk / cw), at byte offset ((16kk) % cw) * 2 of its rows
+          const uint64_t aadv = (uint64_t)(((kk * 16) / cw) * sub16 + (((kk * 16) % cw) >> 3));
+          Wgmma<BN, F16>::template mma<0, 0>(acc, a_hi + aadv, b_hi + badv, (k | kk) != 0);
+          if (NSPLIT == 3) {
+            Wgmma<BN, F16>::template mma<0, 0>(acc, a_lo + aadv, b_hi + badv, 1);
+            Wgmma<BN, F16>::template mma<0, 0>(acc, a_hi + aadv, b_lo + badv, 1);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        // frees the smem stage (the other warpgroup's MMAs on it may still be running: two arrivals)
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[s]);
+      }
+
+      // ---- epilogue: registers -> global ----
       const int mt = tile % m_tiles;
       const int rest = tile / m_tiles;
       const int ncol0 = (rest % n_tiles) * p.block_n;
       const int z = rest / n_tiles;
-      const int gw = (mt % p.tiles_w) * p.tw + w_i;
-      const int gh = ((mt / p.tiles_w) % p.tiles_h) * p.th + h_i;
-      const int gn = (mt / (p.tiles_w * p.tiles_h)) * p.nb + n_i;
-      const bool valid = (row < p.a_rows) && (gw < p.m_w) && (gh < p.m_h) && (gn < p.m_n);
       const int ph_h = p.nphase == 4 ? (z >> 1) : 0, ph_w = p.nphase == 4 ? (z & 1) : 0;
-      float* optr = p.out + (long long)gn * p.out_sn + (long long)(gh * p.omh + p.ooh + ph_h) * p.out_sh +
-                    (long long)(gw * p.omw + p.oow + ph_w) * p.out_sw + ncol0;
-      const uint32_t b = tcount & 1;
-      mbar_wait(&tfull_bar[b], (tcount >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + b * 128 + ((uint32_t)(q * 32) << 16);
-      for (int c0 = 0; c0 < p.block_n; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(tmem_d + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (c0 + 16 >= p.block_n) {   // last read of this accumulator: hand it back before the stores
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[b]);
-        }
-        if (valid && p.stack_slot) {
+      int gw[2], gh[2], gn[2];
+      bool valid[2];
+      float* optr[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        gw[h] = (mt % p.tiles_w) * p.tw + w_i[h];
+        gh[h] = ((mt / p.tiles_w) % p.tiles_h) * p.th + h_i[h];
+        gn[h] = (mt / (p.tiles_w * p.tiles_h)) * p.nb + n_i[h];
+        valid[h] = (row0 + 8 * h < p.a_rows) && (gw[h] < p.m_w) && (gh[h] < p.m_h) && (gn[h] < p.m_n);
+        optr[h] = p.out + (long long)gn[h] * p.out_sn + (long long)(gh[h] * p.omh + p.ooh + ph_h) * p.out_sh +
+                  (long long)(gw[h] * p.omw + p.oow + ph_w) * p.out_sw + ncol0;
+      }
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int c = 8 * i + 2 * quad;    // this thread's column pair (c, c + 1) of the tile
+        if (BN > 16 && 8 * i >= p.block_n) break;   // MMA columns past block_n: not this tile's output
+        if (p.stack_slot) {
           // phase-stacked head: column -> (phase, channel); every phase lands on its own output pixel
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int col = ncol0 + c0 + j;
-            const int ph = col / p.stack_slot, c = col - ph * p.stack_slot;
-            if (ph < 4 && c < p.stack_c) {
-              float v = __uint_as_float(r[j]) * oscale;
-              if (p.bias) v += p.bias[c];
-              float* o = p.out + (long long)gn * p.out_sn + (long long)(gh * p.omh + (ph >> 1)) * p.out_sh +
-                         (long long)(gw * p.omw + (ph & 1)) * p.out_sw + c;
-              *o = apply_act(v, p.act);
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = ncol0 + c + e;
+              const int ph = col / p.stack_slot, ch = col - ph * p.stack_slot;
+              if (ph < 4 && ch < p.stack_c) {
+                float v = acc[4 * i + 2 * h + e] * oscale;
+                if (p.bias) v += p.bias[ch];
+                float* o = p.out + (long long)gn[h] * p.out_sn + (long long)(gh[h] * p.omh + (ph >> 1)) * p.out_sh +
+                           (long long)(gw[h] * p.omw + (ph & 1)) * p.out_sw + ch;
+                *o = apply_act(v, p.act);
+              }
             }
           }
-        } else if (p.stats && ncol0 + c0 >= p.n_valid) {
-          // a 16-column chunk beyond the last output channel (n_valid % 16 == 0 in this mode): nothing to store or sum
         } else if (p.stats) {
-          // InstanceNorm statistics fused into the producer (layers.py:17,33,134): every tile row belongs to image gn
-          // (nb == 1, checked by the host), so the warp's 32 rows reduce to per-column sums of y and y^2 — one fp64
+          // InstanceNorm statistics fused into the producer (layers.py:17,33,134): every tile row belongs to one image
+          // (nb == 1, checked by the host), so the warp's 16 rows reduce to per-column sums of y and y^2 — one fp64
           // atomic pair per column per warp into stats[n][c] = (sum, sum of squares), finalised by stats_finalize.
-          float v[16], sq[16];
+          // n_valid % 16 == 0 in this mode: an 8-column group is either wholly valid or wholly past the last channel.
+          if (ncol0 + 8 * i >= p.n_valid) continue;
+          float v[2][2];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float t = __uint_as_float(r[j]) * oscale;
-            if (p.bias) t += p.bias[ncol0 + c0 + j];
-            v[j] = valid ? t : 0.f;
-          }
-          if (valid) {
+          for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              *reinterpret_cast<float4*>(optr + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) sq[j] = v[j] * v[j];
-          col_sums16(v, lane);
-          col_sums16(sq, lane);
-          if ((lane & 1) == 0) {
-            const int tn = (mt / (p.tiles_w * p.tiles_h)) * p.nb;      // the tile's image (uniform over the CTA)
-            double* st = p.stats + ((long long)tn * p.n_valid + ncol0 + c0 + (lane >> 1)) * 2;
-            atomicAdd(st, (double)v[0]);
-            atomicAdd(st + 1, (double)sq[0]);
-          }
-        } else if (valid) {
-          if (p.vec4 && ncol0 + c0 + 16 <= p.n_valid) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              float4 v;
-              v.x = __uint_as_float(r[j + 0]) * oscale;
-              v.y = __uint_as_float(r[j + 1]) * oscale;
-              v.z = __uint_as_float(r[j + 2]) * oscale;
-              v.w = __uint_as_float(r[j + 3]) * oscale;
-              if (p.bias) {
-                const float4 bb = *reinterpret_cast<const float4*>(p.bias + ncol0 + c0 + j);
-                v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-              }
-              if (p.act) {
-                v.x = apply_act(v.x, p.act); v.y = apply_act(v.y, p.act);
-                v.z = apply_act(v.z, p.act); v.w = apply_act(v.w, p.act);
-              }
-              *reinterpret_cast<float4*>(optr + c0 + j) = v;
+            for (int e = 0; e < 2; ++e) {
+              float t = acc[4 * i + 2 * h + e] * oscale;
+              if (p.bias) t += p.bias[ncol0 + c + e];
+              v[h][e] = valid[h] ? t : 0.f;
             }
-          } else {
+            if (valid[h]) *reinterpret_cast<float2*>(optr[h] + c) = make_float2(v[h][0], v[h][1]);
+          }
+          const float s0 = quad_col_sum(v[0][0] + v[1][0]);
+          const float s1 = quad_col_sum(v[0][1] + v[1][1]);
+          const float q0 = quad_col_sum(v[0][0] * v[0][0] + v[1][0] * v[1][0]);
+          const float q1 = quad_col_sum(v[0][1] * v[0][1] + v[1][1] * v[1][1]);
+          if (lane < 4) {
+            const int tn = (mt / (p.tiles_w * p.tiles_h)) * p.nb;      // the tile's image (uniform over the CTA)
+            double* sp = p.stats + ((long long)tn * p.n_valid + ncol0 + c) * 2;
+            atomicAdd(sp, (double)s0);
+            atomicAdd(sp + 1, (double)q0);
+            atomicAdd(sp + 2, (double)s1);
+            atomicAdd(sp + 3, (double)q1);
+          }
+        } else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int col = ncol0 + c0 + j;
-              if (col < p.n_valid) {
-                float v = __uint_as_float(r[j]) * oscale;
-                if (p.bias) v += p.bias[col];
-                optr[c0 + j] = apply_act(v, p.act);
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+            float v0 = acc[4 * i + 2 * h] * oscale, v1 = acc[4 * i + 2 * h + 1] * oscale;
+            const int col = ncol0 + c;
+            if (p.vec4 && col + 1 < p.n_valid) {
+              if (p.bias) {
+                const float2 bb = *reinterpret_cast<const float2*>(p.bias + col);
+                v0 += bb.x; v1 += bb.y;
               }
+              *reinterpret_cast<float2*>(optr[h] + c) = make_float2(apply_act(v0, p.act), apply_act(v1, p.act));
+            } else {
+              if (col < p.n_valid) optr[h][c] = apply_act(p.bias ? v0 + p.bias[col] : v0, p.act);
+              if (col + 1 < p.n_valid) optr[h][c + 1] = apply_act(p.bias ? v1 + p.bias[col + 1] : v1, p.act);
             }
           }
         }
@@ -397,9 +344,7 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 256);
   if (dyn && threadIdx.x == 0) {
     // the last CTA to finish re-arms the counters for the next launch of this plan (every CTA's tickets are drawn
     // before it gets here; launches of one plan never overlap)
@@ -415,15 +360,13 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
 // ============================================================================
 // wgrad mode
 // ============================================================================
-template <int NSPLIT>
+template <int NSPLIT, int BN, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   using C = Cfg<NSPLIT>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[C::kStages];
   __shared__ __align__(8) uint64_t empty_bar[C::kStages];
-  __shared__ __align__(8) uint64_t accum_bar;
-  __shared__ uint32_t tmem_base_smem;
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -450,25 +393,20 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);    // one arrival per MMA warpgroup
     }
-    mbar_init(&accum_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     for (int pl = 0; pl < C::kPlanes; ++pl) {
       tma_prefetch_desc(&p.tmX[pl]);
       tma_prefetch_desc(&p.tmY[pl]);
     }
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
   if (k_iters > 0) {
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
       if (lane == 0) {
         const TapDesc xt = p.xtaps[tap_i];
         const uint32_t stage_tx = C::kPlanes * (2 * 8192 + y_blocks * y_block_bytes);
@@ -477,7 +415,7 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
         int rot = 0;
         if (p.rot_mode == 1) rot = (int)(((long long)k_iters * blockIdx.y) / gridDim.y);
         else if (p.rot_mode == 2)
-          rot = (int)(((long long)k_iters * ((blockIdx.x + blockIdx.y * gridDim.x) % 148)) / 148);
+          rot = (int)(((long long)k_iters * ((blockIdx.x + blockIdx.y * gridDim.x) % p.sms)) / p.sms);
         for (int it = 0; it < k_iters; ++it) {
           const int s = it % C::kStages;
           const uint32_t ph = (it / C::kStages) & 1;
@@ -519,84 +457,78 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
           }
         }
       }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        const uint32_t idesc = umma_idesc_16(kBlockM, p.block_n, p.x_fmt, p.y_fmt, 1, 1);
-        uint32_t acc = 0;
-        for (int it = 0; it < k_iters; ++it) {
-          const int s = it % C::kStages;
-          const uint32_t ph = (it / C::kStages) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t st = smem_base + s * C::kStageBytes;
-          // MN-major SWIZZLE_128B: LBO = stride between 64-channel blocks (8192 B),
-          // SBO = stride between 8-pixel groups (1024 B)
-          const uint32_t y_layout = umma_layout_of_chunk(ycw);
-          const uint32_t y_sbo = 8u * ycw * 2u;              // 8 pixel rows of the narrow / full atom
-          // merged planes: the 64-channel blocks are [hi 8 KB][lo 8 KB] pairs, 16 KB apart
-          const uint32_t x_lbo = p.x_merged ? 16384u : 8192u;
-          const uint32_t x_lo_off = p.x_merged ? 8192u : (uint32_t)kTileBytes;
-          const uint32_t y_lbo = p.y_merged ? 16384u : (uint32_t)y_block_bytes;
-          const uint32_t y_lo_off = p.y_merged ? 8192u : (uint32_t)kTileBytes;
-          const uint64_t x_hi = umma_smem_desc(st, x_lbo, 1024);
-          // LBO = stride between the N atoms (64-channel blocks, or the grouped taps' narrow blocks)
-          const uint64_t y_hi = umma_smem_desc(st + C::kPlanes * kTileBytes, y_lbo, y_sbo, y_layout);
-          const uint64_t x_lo = umma_smem_desc(st + x_lo_off, x_lbo, 1024);
-          const uint64_t y_lo = umma_smem_desc(st + C::kPlanes * kTileBytes + y_lo_off, y_lbo, y_sbo, y_layout);
+    } else if (warp < kProducerWarp) {
+      // MMA warpgroup wg: X channels [m0 + 64 wg, m0 + 64 wg + 64) = the wg-th 64-channel block of the X tile
+      const int wg = warp >> 2;
+      // The reduction runs over up to millions of pixels per CTA: each 64-pixel stage goes into a fresh tensor-core
+      // accumulator `part` (12 MMA updates), which is then added into `acc` with round-to-nearest fp32 adds — the
+      // tensor core's accumulator truncates, so its error grows with the number of updates it absorbs.
+      float acc[BN / 2], part[BN / 2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {  // 4 x 16 pixels; 16 pixel rows = 2048 B (X), 16 * ycw * 2 B (Y)
-            const uint64_t xadv = (uint64_t)(k * 128);
-            const uint64_t yadv = (uint64_t)((k * 16 * ycw * 2) >> 4);
-            umma_bf16(tmem_base, x_hi + xadv, y_hi + yadv, idesc, acc);
-            acc = 1;
-            if (NSPLIT == 3) {
-              umma_bf16(tmem_base, x_lo + xadv, y_hi + yadv, idesc, 1);
-              umma_bf16(tmem_base, x_hi + xadv, y_lo + yadv, idesc, 1);
-            }
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      // MN-major SWIZZLE_128B: SBO = stride between 8-pixel groups (1024 B); one 64-channel atom per warpgroup
+      const uint32_t y_layout = gmma_layout_of_chunk(ycw);
+      const uint32_t y_sbo = 8u * ycw * 2u;              // 8 pixel rows of the narrow / full atom
+      // merged planes: the 64-channel blocks are [hi 8 KB][lo 8 KB] pairs, 16 KB apart
+      const uint32_t x_lbo = p.x_merged ? 16384u : 8192u;
+      const uint32_t x_lo_off = p.x_merged ? 8192u : (uint32_t)kTileBytes;
+      const uint32_t y_lbo = p.y_merged ? 16384u : (uint32_t)y_block_bytes;
+      const uint32_t y_lo_off = p.y_merged ? 8192u : (uint32_t)kTileBytes;
+      for (int it = 0; it < k_iters; ++it) {
+        const int s = it % C::kStages;
+        const uint32_t ph = (it / C::kStages) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t st = smem_base + s * C::kStageBytes;
+        const uint64_t x_hi = gmma_smem_desc(st + wg * x_lbo, x_lbo, 1024);
+        // LBO = stride between the N atoms (64-channel blocks, or the grouped taps' narrow blocks)
+        const uint64_t y_hi = gmma_smem_desc(st + C::kPlanes * kTileBytes, y_lbo, y_sbo, y_layout);
+        const uint64_t x_lo = gmma_smem_desc(st + x_lo_off + wg * x_lbo, x_lbo, 1024);
+        const uint64_t y_lo = gmma_smem_desc(st + C::kPlanes * kTileBytes + y_lo_off, y_lbo, y_sbo, y_layout);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {  // 4 x 16 pixels; 16 pixel rows = 2048 B (X), 16 * ycw * 2 B (Y)
+          const uint64_t xadv = (uint64_t)(k * 128);
+          const uint64_t yadv = (uint64_t)((k * 16 * ycw * 2) >> 4);
+          Wgmma<BN, F16>::template mma<1, 1>(part, x_hi + xadv, y_hi + yadv, k != 0);
+          if (NSPLIT == 3) {
+            Wgmma<BN, F16>::template mma<1, 1>(part, x_lo + xadv, y_hi + yadv, 1);
+            Wgmma<BN, F16>::template mma<1, 1>(part, x_hi + xadv, y_lo + yadv, 1);
           }
-          umma_commit(&empty_bar[s]);
         }
-        umma_commit(&accum_bar);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(part);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
       }
-    } else {
-      const int q = warp & 3;
-      const int row = m0 + q * 32 + lane;
-      const bool valid = row < p.rows_valid;
-      float* orow = p.out + (long long)row * p.s_row;
-      mbar_wait(&accum_bar, 0);
-      tc_fence_after();
-      for (int c0 = 0; c0 < p.block_n; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (valid) {
-          if (!grouped) {
-            float* optr = orow + p.tap_off[tap_i];
+      const int quad = lane & 3;
+      const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int col = ncol0 + c0 + j;
-              if (col < p.cols_valid)
-                atomicAdd(optr + (long long)col * p.s_col, __uint_as_float(r[j]));
-            }
-          } else {
-            const int b = c0 / ycw;               // which grouped tap this 16-column chunk belongs to
-            if (b < gsize) {
-              float* optr = orow + p.tap_off[tap_i + b];
-              const int cbase = c0 - b * ycw;
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        if (row >= p.rows_valid) continue;
+        float* orow = p.out + (long long)row * p.s_row;
 #pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (cbase + j < p.cols_valid)
-                  atomicAdd(optr + (long long)(cbase + j) * p.s_col, __uint_as_float(r[j]));
+        for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * i + 2 * quad + e;
+            const float v = acc[4 * i + 2 * h + e];
+            if (!grouped) {
+              const int col = ncol0 + c;
+              if (c < p.block_n && col < p.cols_valid) atomicAdd(orow + p.tap_off[tap_i] + (long long)col * p.s_col, v);
+            } else {
+              const int b = c / ycw;               // which grouped tap this column belongs to
+              const int cbase = c - b * ycw;
+              if (b < gsize && cbase < p.cols_valid)
+                atomicAdd(orow + p.tap_off[tap_i + b] + (long long)cbase * p.s_col, v);
             }
           }
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 128);
 }
 
 }  // namespace
@@ -747,8 +679,6 @@ static void pick_patch_conv(int m_n, int m_h, int m_w, int* th, int* tw, int* nb
   }
 }
 
-static int g_smem_attr_done[2][2] = {{0, 0}, {0, 0}};
-
 int sn_tap_gemm_plan_init(TapGemmPlan* plan, const sn_tap_gemm_desc* d) {
   memset(plan, 0, sizeof(*plan));
   TapGemmParams& p = plan->p;
@@ -768,7 +698,7 @@ int sn_tap_gemm_plan_init(TapGemmPlan* plan, const sn_tap_gemm_desc* d) {
              "block_n must be a multiple of 16 in [16,128]");
   SN_REQUIRE(d->a_hi && d->b_hi && d->out, "null operand");
   SN_REQUIRE(d->nsplit == 1 || (d->a_lo && d->b_lo), "nsplit=3 needs lo planes");
-  SN_REQUIRE(d->a_fmt == d->b_fmt, "A and B of one tcgen05.mma must share a 16-bit format (a=%d b=%d)",
+  SN_REQUIRE(d->a_fmt == d->b_fmt, "A and B of one wgmma must share a 16-bit format (a=%d b=%d)",
              d->a_fmt, d->b_fmt);
   int th, tw, nb;
   pick_patch_conv(d->m_n, d->m_h, d->m_w, &th, &tw, &nb);
@@ -864,11 +794,16 @@ int sn_tap_gemm_plan_init(TapGemmPlan* plan, const sn_tap_gemm_desc* d) {
   return SN_OK;
 }
 
-template <int NSPLIT, int CW>
+// MMA N of a plan: the smallest instantiated wgmma N >= block_n (the extra columns are computed and not stored)
+static int mma_n(int block_n) {
+  return block_n <= 16 ? 16 : block_n <= 32 ? 32 : block_n <= 64 ? 64 : block_n <= 96 ? 96 : 128;
+}
+
+template <int NSPLIT, int CW, int BN, bool F16>
 static int launch_tap(const TapGemmPlan* plan, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    SN_CHECK_CUDA(cudaFuncSetAttribute(tap_gemm_kernel<NSPLIT, CW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SN_CHECK_CUDA(cudaFuncSetAttribute(tap_gemm_kernel<NSPLIT, CW, BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        Cfg<NSPLIT>::kSmemBytes));
     attr_done = true;
   }
@@ -886,21 +821,35 @@ static int launch_tap(const TapGemmPlan* plan, cudaStream_t stream) {
   const int total = m_tiles * n_tiles * (int)plan->grid.z;
   if (plan->p.stats) SN_CHECK_CUDA(cudaMemsetAsync(plan->p.stats, 0, plan->stats_bytes, stream));
   const int ctas = one_tile_per_cta ? total : (total < sms ? total : sms);
-  tap_gemm_kernel<NSPLIT, CW><<<ctas, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p, m_tiles, n_tiles, total);
+  tap_gemm_kernel<NSPLIT, CW, BN, F16>
+      <<<ctas, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p, m_tiles, n_tiles, total);
   SN_CHECK_CUDA(cudaGetLastError());
   return SN_OK;
 }
 
-int sn_tap_gemm_plan_launch(const TapGemmPlan* plan, cudaStream_t stream) {
-  const int cw = plan->p.a_chunk;
-  if (plan->nsplit == 3) {
-    if (cw == 64) return launch_tap<3, 64>(plan, stream);
-    if (cw == 32) return launch_tap<3, 32>(plan, stream);
-    return launch_tap<3, 16>(plan, stream);
+template <int NSPLIT, int CW, bool F16>
+static int launch_tap_n(const TapGemmPlan* plan, cudaStream_t stream) {
+  switch (mma_n(plan->p.block_n)) {
+    case 16: return launch_tap<NSPLIT, CW, 16, F16>(plan, stream);
+    case 32: return launch_tap<NSPLIT, CW, 32, F16>(plan, stream);
+    case 64: return launch_tap<NSPLIT, CW, 64, F16>(plan, stream);
+    case 96: return launch_tap<NSPLIT, CW, 96, F16>(plan, stream);
+    default: return launch_tap<NSPLIT, CW, 128, F16>(plan, stream);
   }
-  if (cw == 64) return launch_tap<1, 64>(plan, stream);
-  if (cw == 32) return launch_tap<1, 32>(plan, stream);
-  return launch_tap<1, 16>(plan, stream);
+}
+
+template <int NSPLIT, bool F16>
+static int launch_tap_cw(const TapGemmPlan* plan, cudaStream_t stream) {
+  const int cw = plan->p.a_chunk;
+  if (cw == 64) return launch_tap_n<NSPLIT, 64, F16>(plan, stream);
+  if (cw == 32) return launch_tap_n<NSPLIT, 32, F16>(plan, stream);
+  return launch_tap_n<NSPLIT, 16, F16>(plan, stream);
+}
+
+int sn_tap_gemm_plan_launch(const TapGemmPlan* plan, cudaStream_t stream) {
+  const bool f16 = plan->p.a_fmt == SN_FMT_F16;
+  if (plan->nsplit == 3) return f16 ? launch_tap_cw<3, true>(plan, stream) : launch_tap_cw<3, false>(plan, stream);
+  return f16 ? launch_tap_cw<1, true>(plan, stream) : launch_tap_cw<1, false>(plan, stream);
 }
 
 int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
@@ -937,7 +886,7 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   }
   SN_REQUIRE(d->x_hi && d->y_hi && d->out, "null operand");
   SN_REQUIRE(d->nsplit == 1 || (d->x_lo && d->y_lo), "nsplit=3 needs lo planes");
-  SN_REQUIRE(d->x_fmt == d->y_fmt, "X and Y of one tcgen05.mma must share a 16-bit format (x=%d y=%d)",
+  SN_REQUIRE(d->x_fmt == d->y_fmt, "X and Y of one wgmma must share a 16-bit format (x=%d y=%d)",
              d->x_fmt, d->y_fmt);
   int th, tw, nb;
   pick_patch(d->m_h, d->m_w, 64, &th, &tw, &nb);
@@ -996,6 +945,7 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   const int base_ctas = p.m_tiles * p.n_tiles * grid_y;
   const int total = p.tiles_w * p.tiles_h * p.tiles_n;
   p.rot_mode = 0;
+  p.sms = sm_count;
   if (const char* e = getenv("SN_WGRAD_ROT")) p.rot_mode = atoi(e);
   int ks = d->ksplit;
   if (const char* e = getenv("SN_WGRAD_KSPLIT")) {   // experiment override
@@ -1013,23 +963,32 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   return SN_OK;
 }
 
-int sn_wgrad_plan_launch(const WgradPlan* plan, cudaStream_t stream) {
-  const int idx = plan->nsplit == 3 ? 1 : 0;
-  if (plan->nsplit == 3) {
-    if (!g_smem_attr_done[1][idx]) {
-      SN_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg<3>::kSmemBytes));
-      g_smem_attr_done[1][idx] = 1;
-    }
-    wgrad_gemm_kernel<3><<<plan->grid, kThreads, Cfg<3>::kSmemBytes, stream>>>(plan->p);
-  } else {
-    if (!g_smem_attr_done[1][idx]) {
-      SN_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg<1>::kSmemBytes));
-      g_smem_attr_done[1][idx] = 1;
-    }
-    wgrad_gemm_kernel<1><<<plan->grid, kThreads, Cfg<1>::kSmemBytes, stream>>>(plan->p);
+template <int NSPLIT, int BN, bool F16>
+static int launch_wgrad(const WgradPlan* plan, cudaStream_t stream) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    SN_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<NSPLIT, BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       Cfg<NSPLIT>::kSmemBytes));
+    attr_done = true;
   }
+  wgrad_gemm_kernel<NSPLIT, BN, F16><<<plan->grid, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p);
   SN_CHECK_CUDA(cudaGetLastError());
   return SN_OK;
+}
+
+template <int NSPLIT, bool F16>
+static int launch_wgrad_n(const WgradPlan* plan, cudaStream_t stream) {
+  switch (mma_n(plan->p.block_n)) {
+    case 16: return launch_wgrad<NSPLIT, 16, F16>(plan, stream);
+    case 32: return launch_wgrad<NSPLIT, 32, F16>(plan, stream);
+    case 64: return launch_wgrad<NSPLIT, 64, F16>(plan, stream);
+    case 96: return launch_wgrad<NSPLIT, 96, F16>(plan, stream);
+    default: return launch_wgrad<NSPLIT, 128, F16>(plan, stream);
+  }
+}
+
+int sn_wgrad_plan_launch(const WgradPlan* plan, cudaStream_t stream) {
+  const bool f16 = plan->p.x_fmt == SN_FMT_F16;
+  if (plan->nsplit == 3) return f16 ? launch_wgrad_n<3, true>(plan, stream) : launch_wgrad_n<3, false>(plan, stream);
+  return f16 ? launch_wgrad_n<1, true>(plan, stream) : launch_wgrad_n<1, false>(plan, stream);
 }

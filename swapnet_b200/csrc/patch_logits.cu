@@ -22,7 +22,7 @@ constexpr int kThreads = 256;
 
 inline int grid_for(long long total) {
   long long g = (total + kThreads - 1) / kThreads;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > SN_NUM_SMS * 16) g = SN_NUM_SMS * 16;
   return g < 1 ? 1 : (int)g;
 }
 
@@ -309,7 +309,7 @@ int sn_to_one_fwd(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, lo
   }
   SN_REQUIRE(smem <= 96 * 1024, "to_one_fwd: too many channels (%d)", c);
   long long blocks = (npix + 8 * kPx - 1) / (8 * kPx);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > SN_NUM_SMS * 4) blocks = SN_NUM_SMS * 4;
   to_one_fwd_kernel<16><<<(int)blocks, 256, smem, (cudaStream_t)stream>>>((const uint16_t*)x_hi, (const uint16_t*)x_lo, x_pitch,
                                                                         x_fmt, npix, c, weight, p, p_pitch);
   LAUNCH_CHECK();
@@ -338,7 +338,7 @@ int sn_to_one_wgrad(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, 
     }
   }
   long long blocks = npix / kWgPix;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > SN_NUM_SMS * 4) blocks = SN_NUM_SMS * 4;
   if (blocks < 1) blocks = 1;
   to_one_wgrad_kernel<4><<<(int)blocks, dim3(bx, by), smem, (cudaStream_t)stream>>>(
       (const uint16_t*)x_hi, (const uint16_t*)x_lo, x_pitch, x_fmt, npix, c, d, dw);
@@ -361,7 +361,7 @@ int sn_to_one_dgrad(const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_f
   }
   const long long npix = (long long)n * h * w;
   long long blocks = (npix + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > SN_NUM_SMS * 8) blocks = SN_NUM_SMS * 8;
   to_one_dgrad_kernel<4><<<(int)blocks, kThreads, smem, (cudaStream_t)stream>>>(d, npix, c, weight, dx, dx_pitch);
   LAUNCH_CHECK();
   return SN_OK;

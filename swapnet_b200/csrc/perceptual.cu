@@ -1,4 +1,4 @@
-// swapnet_b200 — element-wise kernels of the VGG16 perceptual loss (sm_100a).
+// swapnet_b200 — element-wise kernels of the VGG16 perceptual loss (sm_90a).
 //
 // Reference: modules/losses/perceptual.py:6-79 as used by models/texture_model.py:68-69,171-176.
 //   get_features:  x <- 2x - 1; five slices of vgg16.features[0:30] (conv3x3+bias+ReLU, MaxPool2d(2));
@@ -19,7 +19,7 @@ constexpr int kThreads = 256;
 
 inline int grid_for(long long total, int threads = kThreads) {
   long long g = (total + threads - 1) / threads;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > SN_NUM_SMS * 16) g = SN_NUM_SMS * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -391,7 +391,7 @@ int sn_feat_loss_fwd_bwd(const float* y_out, int po, const float* y_tgt, int pt,
              "feat_loss: c multiple of 4 and <= 512, pitches multiples of 4");
   const int wpb = kThreads / 32;
   long long blocks = (npix + wpb - 1) / wpb;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > SN_NUM_SMS * 8) blocks = SN_NUM_SMS * 8;
   cudaStream_t st = (cudaStream_t)stream;
   if (c <= 128)
     feat_loss_kernel<1><<<(int)blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx);

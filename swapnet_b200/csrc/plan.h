@@ -57,6 +57,7 @@ struct alignas(64) WgradParams {
   int ngroups;  // > 0: narrow-Y tap groups (grid.y = group)
   int x_merged, y_merged;   // hi+lo of a 64-channel block in one TMA box (see TapGemmParams)
   int rot_mode; // pixel-tile order stagger (0 none, 1 per tap, 2 per CTA)
+  int sms;      // SMs of the device (rot_mode 2)
   short gstart[SN_MAX_TAPS], gsize[SN_MAX_TAPS];
 };
 

@@ -1,4 +1,4 @@
-// swapnet_b200 — fused ROIAlign + channel repack (sm_100a, HBM/latency bound).
+// swapnet_b200 — fused ROIAlign + channel repack (sm_90a, HBM/latency bound).
 //
 // Replaces TextureModule.reshape_rois + torchvision.ops.RoIAlign((128,128), spatial_scale=1,
 // sampling_ratio=1, aligned=False) + the .view() repack of modules/swapnet_modules.py:209-240:
@@ -112,7 +112,7 @@ extern "C" int sn_roi_align_pack_fwd(const float* tex_nchw, int b, int ch, int h
   a.ppitch = plane_pitch; a.pcoff = plane_coff; a.fmt = plane_fmt;
   const long long total = (long long)b * pool * pool * nroi;
   long long grid = (total + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > SN_NUM_SMS * 16) grid = SN_NUM_SMS * 16;
   roi_align_pack_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(a);
   sn_count_launch(1);
   SN_CHECK_CUDA(cudaGetLastError());

@@ -23,6 +23,7 @@ from abc import ABC, abstractmethod
 from argparse import ArgumentParser
 from typing import Optional
 
+import gc
 import os
 
 import torch
@@ -188,6 +189,10 @@ class BaseGAN(BaseModel, ABC):
                         for st in eng.stages:                # break the Stage <-> Engine cycle: buffers free now
                             st.eng = None
                         eng.stages.clear()
+            # A model is a reference cycle (its loss closures, its stages and engines), so the device buffers of a
+            # model the caller has dropped return to the allocator only when the cycle collector runs — which it
+            # schedules by object counts, not by device memory.  Collect before allocating tens of GB for this shape.
+            gc.collect()
             cache[key] = self._build_engines(batch, size)
         else:
             cache[key] = cache.pop(key)                      # most recently used last

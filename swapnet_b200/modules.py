@@ -23,7 +23,7 @@ class _NoEager(nn.Module):
     def forward(self, *a, **k):  # pragma: no cover
         raise RuntimeError(
             f"{type(self).__name__} is a parameter container; the forward/backward of this network "
-            "runs in swapnet_b200.engine (CUDA, sm_100a) — there is no eager fallback")
+            "runs in swapnet_b200.engine (CUDA, sm_90a) — there is no eager fallback")
 
 
 def _slots(conv: nn.Module, index: int, total: int) -> nn.Sequential:

@@ -1,4 +1,4 @@
-"""Data-parallel plumbing (one process per GPU, torch.distributed; NCCL on B200, gloo in CPU tests).
+"""Data-parallel plumbing (one process per GPU, torch.distributed; NCCL on the GPUs, gloo in CPU tests).
 
 The hot path shards over the batch with no data-path collective: convs, InstanceNorm (per sample),
 ROIAlign and the batch-mean losses are all per-sample, so equal shards + gradient averaging

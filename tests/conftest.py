@@ -20,7 +20,7 @@ def record(name: str, value) -> None:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     try:   # the fp64 CPU oracle: as many torch threads as the cgroup quota allows (the GPU boxes show 128 CPUs under
         # a 16-CPU quota; 128 threads there are 8x oversubscribed and ~20x slower)
         import torch

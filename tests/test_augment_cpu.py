@@ -135,6 +135,19 @@ def test_matches_the_reference_function():
         assert np.array_equal(A.per_channel_transform(cloth.numpy(), ops), ref)
 
 
+def test_matches_the_stored_reference_function():
+    """test_matches_the_reference_function against the reference's outputs and generator states stored by
+    tests/tools/make_golden_reference.py (same transforms, label map and seeds)."""
+    z = np.load(os.path.join(os.path.dirname(__file__), "golden", "augment_reference_96.npz"))
+    tf = reference_transform(("hflip", "vflip", "affine", "perspective"))
+    cloth = A.onehot(label_map(96, 96, 7), 19)
+    for seed in (0, 1, 2):
+        random.seed(seed); torch.manual_seed(seed)
+        ops = D.draw_channel_ops(tf, 19, 96, 96)
+        assert rng_digest() == str(z[f"rng_{seed}"])
+        assert np.array_equal(A.per_channel_transform(cloth, ops), z[f"out_{seed}"])
+
+
 def test_golden_fixture_from_the_reference():
     z = np.load(GOLDEN)
     for name in ("all_64", "all_40x56", "affine_64", "flips_64"):

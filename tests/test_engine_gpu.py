@@ -608,6 +608,40 @@ def test_warp_batch16_equals_mean_of_16_single_image_steps_512(mode):
     assert eD < 1e-4 and eG < 1e-4 and el < 1e-5, (eD, eG, el)
 
 
+def test_dropped_model_buffers_are_reused_by_the_next_model():
+    """A model is a reference cycle (loss closures, stages <-> engines): building a model's engines collects dropped
+    models first, so their device buffers are reused instead of piling up (at 512x512, batch 16 one model holds tens of
+    GB of the 80 GB).  Automatic collection is off here so that only the model's own collection can free them."""
+    import gc
+
+    from swapnet_b200.models import create_model
+
+    def build():
+        torch.manual_seed(0)
+        m = create_model(_opt(2, 128))
+        m.setup(m.opt)
+        m.ensure_engines(2, 128)
+        return m
+
+    was_enabled = gc.isenabled()
+    gc.collect()
+    gc.disable()
+    try:
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated()
+        model = build()
+        one = torch.cuda.memory_allocated() - base
+        del model
+        model = build()
+        two = torch.cuda.memory_allocated() - base
+        del model
+    finally:
+        if was_enabled:
+            gc.enable()
+        gc.collect()
+    assert two < 1.5 * one, (one, two)
+
+
 def test_train_loop_protocol():
     """The calls train.py:31-116 makes, in its order, on a two-epoch run whose last batch of each epoch is short (the
     reference's DataLoader has no drop_last, datasets/__init__.py:69): set_input / optimize_parameters /

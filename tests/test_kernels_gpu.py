@@ -191,6 +191,30 @@ BASELINE_CASES = [
 ]
 
 
+def ref_fwd_bwd(kind, x, wt, bias, gy, chunk=4):
+    """fp64 output of ref_forward and its gradients (input, weight, bias) for the output gradient gy, on the GPU,
+    `chunk` images at a time: every image is independent and the weight and bias gradients are sums over the images.
+    At the 512x512 head shape the autograd graph of the whole batch of 16 exceeds the 80 GB of an H100."""
+    d = dev()
+    w = wt.to(d).double().requires_grad_()
+    b = bias.to(d).double().requires_grad_()
+    ys, gxs, gw, gb = [], [], 0, 0
+    for i in range(0, x.shape[0], chunk):
+        xi = x[i:i + chunk].to(d).double().requires_grad_()
+        gyi = gy[i:i + chunk].double()
+        yi = ref_forward(kind, xi, w, b)
+        if kind == "conv3r":   # gradient w.r.t. the PADDED input (what the engine consumes)
+            xp = F.pad(xi.detach(), (1, 1, 1, 1), mode="reflect").requires_grad_()
+            gxi = torch.autograd.grad(F.conv2d(xp, w.detach()), xp, gyi)[0]
+            gwi, gbi = torch.autograd.grad(yi, (w, b), gyi)
+        else:
+            gxi, gwi, gbi = torch.autograd.grad(yi, (xi, w, b), gyi)
+        ys.append(yi.detach())
+        gxs.append(gxi)
+        gw, gb = gw + gwi, gb + gbi
+    return torch.cat(ys), torch.cat(gxs), gw, gb
+
+
 @pytest.mark.parametrize("kind,n,cin,cout,h,w", BASELINE_CASES)
 def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w):
     from swapnet_b200 import ops
@@ -198,24 +222,15 @@ def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w):
     layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
     oh, ow = L.out_hw(kind, h, w)
     d = dev()
-    xr = x.to(d).double().requires_grad_()
-    wr = wt.to(d).double().requires_grad_()
-    br = bias.to(d).double().requires_grad_()
     y = torch.zeros(n, oh, ow, cout, device=d)
     layer.bind_forward(y)
     layer.pack()
     layer.forward()
     torch.cuda.synchronize()
     with torch.backends.cudnn.flags(enabled=True, deterministic=True, allow_tf32=False):
-        yr = ref_forward(kind, xr, wr, br)
-        e_f = relmax(y, nhwc(yr.detach()))
-        gy = torch.randn(yr.shape, generator=torch.Generator().manual_seed(99)).to(d)
-        if kind == "conv3r":   # gradient w.r.t. the PADDED input (what the engine consumes)
-            xp = F.pad(x.to(d).double(), (1, 1, 1, 1), mode="reflect").requires_grad_()
-            gx = torch.autograd.grad(F.conv2d(xp, wt.to(d).double()), xp, gy.double())[0]
-            gw, gb = torch.autograd.grad(yr, (wr, br), gy.double())
-        else:
-            gx, gw, gb = torch.autograd.grad(yr, (xr, wr, br), gy.double())
+        gy = torch.randn((n, cout, oh, ow), generator=torch.Generator().manual_seed(99)).to(d)
+        yr, gx, gw, gb = ref_fwd_bwd(kind, x, wt, bias, gy)
+        e_f = relmax(y, nhwc(yr))
     dyc = L.padc(cout) if layer.x.c >= 64 else L.pad64(cout)
     dy = ops.Planes(n, oh, ow, dyc, d, fmt=ops.FMT_BF16)
     if cout * 33 * 4 > 48 * 1024:

@@ -158,6 +158,39 @@ def test_oracle_is_bit_identical_to_reference_modules():
     assert all(torch.equal(a.state_dict()[k], b.state_dict()[k]) for k in a.state_dict())
 
 
+def close_sums(t, want, tol):
+    got = (float(t.double().sum()), float(t.double().abs().sum()))
+    assert all(abs(x - y) <= tol * max(1.0, abs(y)) for x, y in zip(got, want)), (got, want)
+
+
+def test_oracle_matches_the_stored_reference_modules():
+    """test_oracle_is_bit_identical_to_reference_modules against the reference's outputs stored by
+    tests/tools/make_golden_reference.py (same seeds and inputs); the host's CPU kernels may round differently, hence
+    the fp32-rounding tolerance instead of bit equality."""
+    g = torch.load(os.path.join(GOLD, "reference_modules.pt"))
+    torch.manual_seed(0)
+    G = M.WarpModule(); M.init_weights(G, "kaiming")
+    D = M.NLayerDiscriminator(22, 64, 3, "instance"); M.init_weights(D, "kaiming")
+    body, inp, _ = synth_warp_batch(2, 64)
+    with torch.no_grad():
+        fakes = ON.warp_forward(G.state_dict(), body, inp)
+        pred = ON.patchgan_forward(D.state_dict(), torch.cat((body, fakes), 1))
+    assert relmax(fakes[:, :, ::4, ::4], g["warp_fakes_sub"]) < 1e-6 and relmax(pred, g["patchgan_pred"]) < 1e-6
+    close_sums(fakes, g["warp_fakes_sums"], 1e-6)
+    torch.manual_seed(0)
+    T = M.TextureModule(3, 19, 12, "instance", 0.5, 128); M.init_weights(T, "kaiming")
+    tex, rois, cloth, _ = synth_texture_batch(2, 128)
+    with torch.no_grad():
+        out = ON.texture_forward(T.state_dict(), tex, rois, cloth)
+    assert relmax(out[:, :, ::4, ::4], g["texture_fakes_sub"]) < 1e-6
+    close_sums(out, g["texture_fakes_sums"], 1e-6)
+    torch.manual_seed(3)
+    b = M.WarpModule(); M.init_weights(b, "kaiming")
+    assert list(b.state_dict()) == g["warp_state_keys"]
+    for k, v in b.state_dict().items():
+        close_sums(v, g["warp_seed3_sums"][k], 0.0)
+
+
 def seeded_vgg_features_sd(seed=1234):
     """The stand-in for the unobtainable `vgg16(pretrained=True)`: torchvision's own constructor
     (kaiming_normal fan_out convs, zero bias) under a fixed seed (SURVEY App. C)."""
@@ -198,6 +231,22 @@ def test_perceptual_oracle_is_bit_identical_to_reference():
     c, s_ = ON.perceptual_loss(sd, out, tgt, True)
     (c * 20 + s_ * 1e-8).backward()
     assert torch.equal(c, c_ref) and torch.equal(s_, s_ref) and torch.equal(out.grad, g_ref)
+
+
+def test_perceptual_oracle_matches_the_stored_reference():
+    """test_perceptual_oracle_is_bit_identical_to_reference against the reference's values stored by
+    tests/tools/make_golden_reference.py (same inputs)."""
+    g = torch.load(os.path.join(GOLD, "reference_modules.pt"))["perceptual"]
+    sd = seeded_vgg_features_sd()
+    gen = torch.Generator().manual_seed(5)
+    out = torch.rand(2, 3, 64, 64, generator=gen).requires_grad_()
+    tgt = torch.rand(2, 3, 64, 64, generator=gen)
+    c, s = ON.perceptual_loss(sd, out, tgt, True)
+    (c * 20 + s * 1e-8).backward()
+    assert abs(float(c) - g["content"]) <= 1e-6 * abs(g["content"])
+    assert abs(float(s) - g["style"]) <= 1e-6 * abs(g["style"])
+    assert relmax(out.grad[:, :, ::4, ::4], g["grad_sub"]) < 1e-5
+    close_sums(out.grad, g["grad_sums"], 1e-5)
 
 
 def test_perceptual_oracle_matches_golden():
