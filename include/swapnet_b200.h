@@ -143,6 +143,9 @@ int sn_plan_run(const sn_plan* plan, void* stream);
 void sn_plan_destroy(sn_plan* plan);
 /* 1 when the plan accumulates the fused InstanceNorm statistics requested through sn_tap_gemm_desc.stats */
 int sn_plan_has_stats(const sn_plan* plan);
+/* launch geometry of a plan, for per-plan timing tables: out[0] = kind (0 tap GEMM, 1 weight gradient), then
+ * tap GEMM: M tiles, N tiles, phases, block_n, A row chunk; weight gradient: grid x, y, z, block_n, Y row chunk */
+int sn_plan_geometry(const sn_plan* plan, int* out);
 
 /* ------------------------------------------------------------------------------------------
  * operand packing

@@ -122,6 +122,7 @@ SIGNATURES = {
     "sn_plan_run": (_I, [_VP, _VP]),
     "sn_plan_destroy": (None, [_VP]),
     "sn_plan_has_stats": (_I, [_VP]),
+    "sn_plan_geometry": (_I, [_VP, C.POINTER(C.c_int)]),
     "sn_stats_finalize": (_I, [_VP, _I, _I, _F, _VP]),
     "sn_pack_planes": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_pack_concat": (_I, [_VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),

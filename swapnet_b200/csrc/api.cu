@@ -74,6 +74,18 @@ int sn_plan_run(const sn_plan* plan, void* stream) {
 
 int sn_plan_has_stats(const sn_plan* plan) { return plan && plan->kind == 0 && plan->tg.p.stats != nullptr; }
 
+int sn_plan_geometry(const sn_plan* plan, int* out) {
+  SN_REQUIRE(plan && out, "null argument");
+  const dim3 g = plan->kind == 0 ? plan->tg.grid : plan->wg.grid;
+  out[0] = plan->kind;
+  out[1] = (int)g.x;
+  out[2] = (int)g.y;
+  out[3] = (int)g.z;
+  out[4] = plan->kind == 0 ? plan->tg.p.block_n : plan->wg.p.block_n;
+  out[5] = plan->kind == 0 ? plan->tg.p.a_chunk : plan->wg.p.y_chunk;
+  return SN_OK;
+}
+
 void sn_plan_destroy(sn_plan* plan) {
   if (plan && plan->kind == 0 && plan->tg.p.tile_counter) cudaFree(plan->tg.p.tile_counter);
   delete plan;

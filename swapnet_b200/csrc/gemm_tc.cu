@@ -71,10 +71,19 @@ __device__ __forceinline__ float quad_col_sum(float v) {
 template <int NSPLIT, int CW, int BN, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, const int n_tiles, const int total_tiles) {
-  // Persistent: one CTA per SM walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... (M tile fastest, then N tile,
+  // Persistent: one CTA per SM walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tile fastest, then M tile,
   // then output-parity phase).  The smem ring keeps running across tiles, so the producer loads the next tile's
   // stages while the MMA warpgroups run the epilogue of the current one, and the pipeline prologue is paid once per
   // CTA instead of once per tile.
+  // N tile fastest: the resident CTAs cover all N tiles of ~132 / n_tiles M tiles, so the activation rows they read
+  // (~10 MB for a resblock conv) stay in L2 from one tap to the next.  M tile fastest spread them over 132 M tiles:
+  // the whole 75 MB operand, beyond the 50 MB L2, so every tap re-read it from HBM.
+  const auto tile_coords = [&](int tile, int& mt, int& nt, int& z) {
+    nt = tile % n_tiles;
+    const int rest = tile / n_tiles;
+    mt = rest % m_tiles;
+    z = rest / m_tiles;
+  };
   using C = Cfg<NSPLIT>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[C::kStages];
@@ -134,10 +143,10 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
           mbar_arrive(&tr_full[slot]);
         }
         if (tile >= total_tiles) break;
-        const int mt = tile % m_tiles;
-        const int rest = tile / m_tiles;
-        const int ncol0 = (rest % n_tiles) * p.block_n;
-        const int tap0 = (rest / n_tiles) * tpp;
+        int mt, nt, z;
+        tile_coords(tile, mt, nt, z);
+        const int ncol0 = nt * p.block_n;
+        const int tap0 = z * tpp;
         const int w0 = (mt % p.tiles_w) * p.tw;
         const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.th;
         const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.nb;
@@ -254,10 +263,9 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
       }
 
       // ---- epilogue: registers -> global ----
-      const int mt = tile % m_tiles;
-      const int rest = tile / m_tiles;
-      const int ncol0 = (rest % n_tiles) * p.block_n;
-      const int z = rest / n_tiles;
+      int mt, nt, z;
+      tile_coords(tile, mt, nt, z);
+      const int ncol0 = nt * p.block_n;
       const int ph_h = p.nphase == 4 ? (z >> 1) : 0, ph_w = p.nphase == 4 ? (z & 1) : 0;
       int gw[2], gh[2], gn[2];
       bool valid[2];
