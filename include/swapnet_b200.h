@@ -214,6 +214,21 @@ int sn_plane_stats(const float* y, int pitch, int n, int hw, int c, float eps, d
                    void* stream);
 /* (sum, sum of squares) over hw pixels -> (mean, 1/sqrt(var_biased + eps)) in place, `count` = n*c pairs */
 int sn_stats_finalize(double* stats, int count, int hw, float eps, void* stream);
+/* per-(n,c) (sum, sum of squares) over the plane, accumulated in fp64, without sn_stats_finalize's conversion */
+int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream);
+
+/* BatchNorm2d(affine, track_running_stats) statistics (pix2pix / PatchGAN `--norm batch`).  The n samples form `groups`
+ * consecutive groups of n/groups samples, each normalised as a call of its own (the discriminator's fake and real
+ * halves).  Reductions over the samples run in sample order on one thread per channel: no atomics.
+ * sn_bn_finalize (train mode): stats[n][c] = (sum, sum of squares) over hw pixels (a fused GEMM epilogue or
+ * sn_plane_sums) -> (mean, 1/sqrt(var_biased + eps)) of the sample's group, in place; then, group after group,
+ * running_mean/var <- (1 - momentum) * running + momentum * (mean, unbiased variance) and num_batches_tracked += groups
+ * (running buffers and counter may be NULL: not tracked).
+ * sn_bn_eval_stats (eval mode): stats[n][c] = (running_mean, 1/sqrt(running_var + eps)); nothing is updated. */
+int sn_bn_finalize(double* stats, int n, int c, int groups, int hw, float eps, float momentum, float* running_mean,
+                   float* running_var, long long* num_batches_tracked, void* stream);
+int sn_bn_eval_stats(double* stats, int n, int c, const float* running_mean, const float* running_var, float eps,
+                     void* stream);
 
 typedef struct sn_norm_act_desc {
   const float* y; int y_pitch;           /* conv output, [n, h, w, c] */
@@ -236,6 +251,8 @@ typedef struct sn_norm_act_desc {
                                             of one wgmma must share a format) */
   int out_reflect_pad;                   /* 1: planes are [n, h+2, w+2] with ReflectionPad2d(1) */
   float* out_f32; int f32_pitch;         /* optional fp32 copy (residual stream) */
+  const float* gamma; const float* beta; /* optional [c] BatchNorm weight / bias: the normalised value is
+                                            gamma * xhat + beta (activation gate included); needs stats, c % 4 == 0 */
 } sn_norm_act_desc;
 int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream);
 
@@ -262,6 +279,11 @@ typedef struct sn_norm_act_bwd_desc {
   int dy_fmt;
   float* bias_grad;                      /* optional [c], c in {256, 512, 1024}: += sum over pixels of dL/dy (the bias
                                             gradient of the conv that produced y), fused into the apply pass */
+  const float* gamma; const float* beta; /* BatchNorm (both NULL: InstanceNorm / none).  stats hold the (mean, rstd) of
+                                            sn_bn_finalize or sn_bn_eval_stats */
+  int bn_groups;                         /* sample groups of the forward call (sn_bn_finalize) */
+  int bn_train;                          /* 1: batch statistics (dL/dy subtracts the group means); 0: running statistics */
+  float* gamma_grad; float* beta_grad;   /* optional [c]: += d(loss)/d(gamma), d(loss)/d(beta) */
 } sn_norm_act_bwd_desc;
 int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream);
 

@@ -87,6 +87,7 @@ class SnNormActDesc(C.Structure):
         ("out_fmt", C.c_int), ("out2_hi", C.c_void_p), ("out2_lo", C.c_void_p), ("out2_fmt", C.c_int),
         ("out_reflect_pad", C.c_int),
         ("out_f32", C.c_void_p), ("f32_pitch", C.c_int),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p),
     ]
 
 
@@ -107,6 +108,8 @@ class SnNormActBwdDesc(C.Structure):
         ("gstats", C.c_void_p),
         ("dy_hi", C.c_void_p), ("dy_lo", C.c_void_p), ("dy_pitch", C.c_int), ("dy_coff", C.c_int),
         ("dy_fmt", C.c_int), ("bias_grad", C.c_void_p),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("bn_groups", C.c_int), ("bn_train", C.c_int),
+        ("gamma_grad", C.c_void_p), ("beta_grad", C.c_void_p),
     ]
 
 
@@ -124,6 +127,9 @@ SIGNATURES = {
     "sn_plan_has_stats": (_I, [_VP]),
     "sn_plan_geometry": (_I, [_VP, C.POINTER(C.c_int)]),
     "sn_stats_finalize": (_I, [_VP, _I, _I, _F, _VP]),
+    "sn_plane_sums": (_I, [_VP, _I, _I, _I, _I, _VP, _VP]),
+    "sn_bn_finalize": (_I, [_VP, _I, _I, _I, _I, _F, _F, _VP, _VP, _VP, _VP]),
+    "sn_bn_eval_stats": (_I, [_VP, _I, _I, _VP, _VP, _F, _VP]),
     "sn_pack_planes": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_pack_concat": (_I, [_VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "sn_weight_scale": (_I, [_VP, _LL, _VP, _VP]),

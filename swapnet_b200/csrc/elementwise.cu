@@ -546,6 +546,78 @@ __global__ void gstats_finalize_kernel(double* g, int count, int hw) {
   }
 }
 
+// ---------------------------------------------------------------------------------
+// BatchNorm2d (affine, tracked running statistics) on top of the per-(n, c) sums.  The N samples form `groups`
+// consecutive groups of N/groups samples, each normalised with its own statistics as if it were a call of its own
+// (the discriminator's fake and real halves).  One thread per channel sums the samples in index order: no atomics,
+// the same result on every run.
+// ---------------------------------------------------------------------------------
+// stats[n][c] = (sum y, sum y^2) -> (mean_G, rstd_G) of the sample's group; running buffers updated group by group
+__global__ void bn_finalize_kernel(double* stats, int N, int C, int groups, int hw, double eps, float momentum,
+                                   float* run_mean, float* run_var, long long* num_batches) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c == 0 && num_batches) *num_batches += groups;
+  if (c >= C) return;
+  const int per = N / groups;
+  const double cnt = (double)per * hw;
+  float rm = run_mean ? run_mean[c] : 0.f, rv = run_var ? run_var[c] : 0.f;
+  for (int gi = 0; gi < groups; ++gi) {
+    double s1 = 0.0, s2 = 0.0;
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      s1 += stats[((long long)n * C + c) * 2];
+      s2 += stats[((long long)n * C + c) * 2 + 1];
+    }
+    const double mean = s1 / cnt;
+    double var = s2 / cnt - mean * mean;
+    if (var < 0) var = 0;
+    const double rstd = rsqrt(var + eps);
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      stats[((long long)n * C + c) * 2] = mean;
+      stats[((long long)n * C + c) * 2 + 1] = rstd;
+    }
+    // torch: running <- (1 - momentum) * running + momentum * stat, the variance stat unbiased (n / (n - 1))
+    rm = (float)((1.0 - momentum) * rm + momentum * mean);
+    rv = (float)((1.0 - momentum) * rv + momentum * (cnt > 1 ? var * cnt / (cnt - 1) : var));
+  }
+  if (run_mean) run_mean[c] = rm;
+  if (run_var) run_var[c] = rv;
+}
+// eval mode: stats[n][c] = (running_mean, 1/sqrt(running_var + eps))
+__global__ void bn_eval_stats_kernel(double* stats, int N, int C, const float* run_mean, const float* run_var,
+                                     double eps) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N * C) {
+    const int c = i % C;
+    stats[2 * i] = run_mean[c];
+    stats[2 * i + 1] = rsqrt((double)run_var[c] + eps);
+  }
+}
+// g[n][c] = (sum g, sum g*xhat) -> the group means the apply pass subtracts (train) or zeros (eval: the statistics are
+// constants); d(gamma) += sum g*xhat, d(beta) += sum g over every sample
+__global__ void bn_bwd_group_kernel(double* g, int N, int C, int groups, int hw, int train, float* dgamma,
+                                    float* dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int per = N / groups;
+  const double cnt = (double)per * hw;
+  double tb = 0.0, tg = 0.0;
+  for (int gi = 0; gi < groups; ++gi) {
+    double s1 = 0.0, s2 = 0.0;
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      s1 += g[((long long)n * C + c) * 2];
+      s2 += g[((long long)n * C + c) * 2 + 1];
+    }
+    tb += s1;
+    tg += s2;
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      g[((long long)n * C + c) * 2] = train ? s1 / cnt : 0.0;
+      g[((long long)n * C + c) * 2 + 1] = train ? s2 / cnt : 0.0;
+    }
+  }
+  if (dbeta) dbeta[c] += (float)tb;
+  if (dgamma) dgamma[c] += (float)tg;
+}
+
 
 // bias gradient: db[c] = sum over pixels of dy (dy carried as split planes)
 __global__ void bias_grad_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo,
@@ -641,6 +713,7 @@ struct NormActFwdArgs {
   uint16_t* hi; uint16_t* lo; int out_pitch, out_coff, reflect, fmt;
   uint16_t* hi2; uint16_t* lo2; int fmt2;
   float* f32; int f32_pitch;
+  const float* gamma; const float* beta;   // BatchNorm affine (the AFF kernel instantiations): out = gamma*xhat + beta
 };
 
 __device__ __forceinline__ float act_fwd(float v, int act, float slope) {
@@ -772,6 +845,7 @@ struct NormActBwdArgs {
   double* gstats;
   uint16_t* hi; uint16_t* lo; int dy_pitch, dy_coff, fmt;
   float* bias_grad;   // optional [C]: += per-channel sums of the dy written (the conv's bias gradient)
+  const float* gamma; const float* beta;   // BatchNorm affine (AFF instantiations): the gate is on gamma*xhat + beta
 };
 
 // gradient w.r.t. xhat (before the InstanceNorm backward), and xhat itself
@@ -1218,16 +1292,22 @@ __device__ __forceinline__ void store_split4(uint16_t* hi, uint16_t* lo, long lo
   if (lo) *reinterpret_cast<uint2*>(lo + off) = pl;
 }
 
-template <int MINB>
+template <int MINB, bool AFF = false>
 __global__ void __launch_bounds__(256, MINB) norm_act_fwd_v4_kernel(const NormActFwdArgs a) {
-  extern __shared__ float sm[];  // mean[C], rstd[C]
+  extern __shared__ float sm[];  // mean[C], rstd[C] (+ gamma[C], beta[C] when AFF)
   float* s_mean = sm;
   float* s_rstd = sm + a.C;
+  float* s_gam = sm + 2 * a.C;
+  float* s_bet = sm + 3 * a.C;
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
   const int n = blockIdx.y;
   for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
     s_mean[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2] : 0.f;
     s_rstd[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2 + 1] : 1.f;
+    if constexpr (AFF) {
+      s_gam[c] = a.gamma[c];
+      s_bet[c] = a.beta[c];
+    }
   }
   __syncthreads();
   const int HW = a.H * a.W, Q = a.C >> 2;
@@ -1244,6 +1324,7 @@ __global__ void __launch_bounds__(256, MINB) norm_act_fwd_v4_kernel(const NormAc
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       float t = (v[j] - s_mean[c + j]) * s_rstd[c + j];
+      if constexpr (AFF) t = t * s_gam[c + j] + s_bet[c + j];
       t = act_fwd(t, a.act, a.slope);
       if (a.drop_thresh) {
         const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
@@ -1326,9 +1407,11 @@ __device__ __forceinline__ float4 gather_grad4(const GradSrcs& g, int n, int h, 
   return acc;
 }
 
-// g (w.r.t. xhat) and xhat for a channel quad
+// g (w.r.t. the normalised value, gamma*xhat + beta when AFF) and xhat for a channel quad
+template <bool AFF = false>
 __device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned long long seed, int n, int p, int c,
-                                           const float* mean, const float* rstd, float g[4], float xh[4]) {
+                                           const float* mean, const float* rstd, float g[4], float xh[4],
+                                           const float* gam = nullptr, const float* bet = nullptr) {
   const int HW = a.H * a.W;
   const long long pix = (long long)n * HW + p;
   const int h = p / a.W, w = p - h * a.W;
@@ -1347,7 +1430,10 @@ __device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned lon
     const float gg[4] = {gv.x, gv.y, gv.z, gv.w};
     const int act = s.act >= 0 ? s.act : a.act;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) g[j] += gg[j] * act_grad(xh[j], act, a.slope);
+    for (int j = 0; j < 4; ++j) {
+      if constexpr (AFF) g[j] += gg[j] * act_grad(xh[j] * gam[j] + bet[j], act, a.slope);
+      else g[j] += gg[j] * act_grad(xh[j], act, a.slope);
+    }
   }
   if (a.drop_thresh) {
 #pragma unroll
@@ -1360,7 +1446,7 @@ __device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned lon
 
 // grid (ceil(Q/bx), slabs, N), block (bx, 256/bx) with bx = min(32, pow2 >= Q): thread = channel quad,
 // strided over pixels (C = 64 layers — the largest tensors — use bx = 16, 16 pixel rows)
-template <int MINB>
+template <int MINB, bool AFF = false>
 __global__ void __launch_bounds__(256, MINB) norm_act_bwd_reduce_v4_kernel(const NormActBwdArgs a) {
   __shared__ float red[256][8];
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
@@ -1372,15 +1458,19 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_reduce_v4_kernel(const
   const int p0 = blockIdx.y * per, p1 = min(HW, p0 + per);
   float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
   if (c < a.C) {
-    float mean[4], rstd[4];
+    float mean[4], rstd[4], gam[4], bet[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       mean[j] = (float)a.stats[((long long)n * a.C + c + j) * 2];
       rstd[j] = (float)a.stats[((long long)n * a.C + c + j) * 2 + 1];
+      if constexpr (AFF) {
+        gam[j] = a.gamma[c + j];
+        bet[j] = a.beta[c + j];
+      }
     }
     for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
       float g[4], xh[4];
-      grad_xhat4(a, seed, n, p, c, mean, rstd, g, xh);
+      grad_xhat4<AFF>(a, seed, n, p, c, mean, rstd, g, xh, gam, bet);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         s1[j] += g[j];
@@ -1409,13 +1499,15 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_reduce_v4_kernel(const
   }
 }
 
-template <int MINB>
+template <int MINB, bool AFF = false>
 __global__ void __launch_bounds__(256, MINB) norm_act_bwd_apply_v4_kernel(const NormActBwdArgs a) {
-  extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x C
+  extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x C (+ gamma, beta when AFF)
   float* s_mean = sm;
   float* s_rstd = sm + a.C;
   float* s_m1 = sm + 2 * a.C;
   float* s_m2 = sm + 3 * a.C;
+  float* s_gam = sm + 4 * a.C;
+  float* s_bet = sm + 5 * a.C;
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
   const int n = blockIdx.y;
   for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
@@ -1424,6 +1516,10 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_apply_v4_kernel(const 
     s_rstd[c] = a.stats ? (float)a.stats[k + 1] : 1.f;
     s_m1[c] = a.stats ? (float)a.gstats[k] : 0.f;
     s_m2[c] = a.stats ? (float)a.gstats[k + 1] : 0.f;
+    if constexpr (AFF) {
+      s_gam[c] = a.gamma[c];
+      s_bet[c] = a.beta[c];
+    }
   }
   __syncthreads();
   const int HW = a.H * a.W, Q = a.C >> 2;
@@ -1436,8 +1532,11 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_apply_v4_kernel(const 
     const int p = p0 + pl;
     const int c = (i - pl * Q) << 2;
     float g[4], xh[4];
-    grad_xhat4(a, seed, n, p, c, s_mean + c, s_rstd + c, g, xh);
-    if (a.stats) {
+    grad_xhat4<AFF>(a, seed, n, p, c, s_mean + c, s_rstd + c, g, xh, s_gam + c, s_bet + c);
+    if constexpr (AFF) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) g[j] = s_gam[c + j] * s_rstd[c + j] * (g[j] - s_m1[c + j] - xh[j] * s_m2[c + j]);
+    } else if (a.stats) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) g[j] = s_rstd[c + j] * (g[j] - s_m1[c + j] - xh[j] * s_m2[c + j]);
     }
@@ -1947,6 +2046,39 @@ int sn_plane_stats(const float* y, int pitch, int n, int hw, int c, float eps, d
   return SN_OK;
 }
 
+int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream) {
+  SN_REQUIRE(y && stats, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  SN_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * c, st));
+  const int cg = (c + 31) / 32;
+  int slabs = (SN_NUM_SMS * 4 + n * cg - 1) / (n * cg);
+  if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
+  if (slabs < 1) slabs = 1;
+  plane_stats_kernel<<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_bn_finalize(double* stats, int n, int c, int groups, int hw, float eps, float momentum, float* running_mean,
+                   float* running_var, long long* num_batches_tracked, void* stream) {
+  SN_REQUIRE(stats && n >= 1 && c >= 1 && hw >= 1, "bn_finalize: bad arguments");
+  SN_REQUIRE(groups >= 1 && n % groups == 0, "bn_finalize: %d samples do not split into %d groups", n, groups);
+  SN_REQUIRE((running_mean == nullptr) == (running_var == nullptr), "bn_finalize: running mean and variance go together");
+  bn_finalize_kernel<<<(c + 127) / 128, 128, 0, (cudaStream_t)stream>>>(stats, n, c, groups, hw, (double)eps, momentum,
+                                                                       running_mean, running_var, num_batches_tracked);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_bn_eval_stats(double* stats, int n, int c, const float* running_mean, const float* running_var, float eps,
+                     void* stream) {
+  SN_REQUIRE(stats && running_mean && running_var && n >= 1 && c >= 1, "bn_eval_stats: bad arguments");
+  bn_eval_stats_kernel<<<(n * c + 255) / 256, 256, 0, (cudaStream_t)stream>>>(stats, n, c, running_mean, running_var,
+                                                                              (double)eps);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
 int sn_stats_finalize(double* stats, int count, int hw, float eps, void* stream) {
   SN_REQUIRE(stats && count >= 1 && hw >= 1, "stats_finalize: bad arguments");
   stats_finalize_kernel<<<(count + 255) / 256, 256, 0, (cudaStream_t)stream>>>(stats, count, hw, (double)eps);
@@ -1972,6 +2104,9 @@ int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream) {
   a.fmt = d->out_fmt;
   a.hi2 = (uint16_t*)d->out2_hi; a.lo2 = (uint16_t*)d->out2_lo; a.fmt2 = d->out2_fmt;
   a.f32 = d->out_f32; a.f32_pitch = d->f32_pitch;
+  a.gamma = d->gamma; a.beta = d->beta;
+  SN_REQUIRE((d->gamma == nullptr) == (d->beta == nullptr), "norm_act_fwd: gamma and beta go together");
+  SN_REQUIRE(!d->gamma || d->stats, "norm_act_fwd: the affine (BatchNorm) variant needs stats");
   const bool vec = (d->c % 4 == 0) && al16(d->y) && (d->y_pitch % 4 == 0) &&
                    (!d->residual || (al16(d->residual) && d->res_pitch % 4 == 0)) &&
                    (!d->out_f32 || (al16(d->out_f32) && d->f32_pitch % 4 == 0)) &&
@@ -1979,7 +2114,13 @@ int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream) {
                                    ((uintptr_t)d->out_lo & 7) == 0 && ((uintptr_t)d->out2_hi & 7) == 0 &&
                                    ((uintptr_t)d->out2_lo & 7) == 0)) &&
                    d->c <= 4096;
-  if (vec) {
+  if (d->gamma) {
+    SN_REQUIRE(vec, "norm_act_fwd: the affine (BatchNorm) variant needs c %% 4 == 0 and 16-byte aligned rows (c=%d)", d->c);
+    // mean, rstd, gamma, beta in shared memory: 4 * c floats within the 48 KB a launch gets without opting in
+    SN_REQUIRE(d->c <= 3072, "norm_act_fwd: the affine (BatchNorm) variant supports at most 3072 channels (c=%d)", d->c);
+    dim3 grid(vslabs(d->h * d->w, d->n), d->n);
+    norm_act_fwd_v4_kernel<4, true><<<grid, 256, 4 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
+  } else if (vec) {
     dim3 grid(vslabs(d->h * d->w, d->n), d->n);
     if (ew_use_v4()) {
       const int mb = ew_min_blocks();
@@ -2027,10 +2168,16 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
   a.hi = (uint16_t*)d->dy_hi; a.lo = (uint16_t*)d->dy_lo;
   a.dy_pitch = d->dy_pitch; a.dy_coff = d->dy_coff; a.fmt = d->dy_fmt;
   a.bias_grad = d->bias_grad;
+  a.gamma = d->gamma; a.beta = d->beta;
+  const bool aff = d->gamma != nullptr;
+  SN_REQUIRE((d->gamma == nullptr) == (d->beta == nullptr), "norm_act_bwd: gamma and beta go together");
+  SN_REQUIRE(!aff || (d->stats && d->bn_groups >= 1 && d->n % d->bn_groups == 0 && !d->bias_grad),
+             "norm_act_bwd: the BatchNorm variant needs stats, bn_groups dividing n, and no fused bias gradient");
   const int hw = d->h * d->w;
   const bool vec = (d->c % 4 == 0) && al16(d->y) && (d->y_pitch % 4 == 0) && srcs_vec_ok(a.g) &&
                    (d->dy_pitch % 4 == 0) && (d->dy_coff % 4 == 0) && ((uintptr_t)d->dy_hi & 7) == 0 &&
                    ((uintptr_t)d->dy_lo & 7) == 0 && d->c <= 2048;
+  SN_REQUIRE(!aff || vec, "norm_act_bwd: the BatchNorm variant needs c %% 4 == 0 and 16-byte aligned rows (c=%d)", d->c);
   if (d->stats) {
     SN_REQUIRE(d->gstats, "InstanceNorm backward needs gstats scratch");
     SN_CHECK_CUDA(cudaMemsetAsync(d->gstats, 0, sizeof(double) * 2 * d->n * d->c, st));
@@ -2041,7 +2188,8 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       int slabs = (SN_NUM_SMS * 6 + d->n * qg - 1) / (d->n * qg);
       if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
       if (slabs < 1) slabs = 1;
-      if (ew_use_v4()) {
+      if (aff) norm_act_bwd_reduce_v4_kernel<4, true><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
+      else if (ew_use_v4()) {
         const int mb = ew_min_blocks();
         if (mb == 5) norm_act_bwd_reduce_v4_kernel<5><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
         else if (mb == 6) norm_act_bwd_reduce_v4_kernel<6><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
@@ -2056,10 +2204,17 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       norm_act_bwd_reduce_kernel<<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
     }
     LAUNCH_CHECK();
-    gstats_finalize_kernel<<<(d->n * d->c + 255) / 256, 256, 0, st>>>(d->gstats, d->n * d->c, hw);
+    if (aff)
+      bn_bwd_group_kernel<<<(d->c + 127) / 128, 128, 0, st>>>(d->gstats, d->n, d->c, d->bn_groups, hw, d->bn_train,
+                                                              d->gamma_grad, d->beta_grad);
+    else
+      gstats_finalize_kernel<<<(d->n * d->c + 255) / 256, 256, 0, st>>>(d->gstats, d->n * d->c, hw);
     LAUNCH_CHECK();
   }
-  if (vec) {
+  if (aff) {
+    dim3 grid(vslabs(hw, d->n), d->n);
+    norm_act_bwd_apply_v4_kernel<4, true><<<grid, 256, 6 * d->c * sizeof(float), st>>>(a);
+  } else if (vec) {
     dim3 grid(vslabs(hw, d->n), d->n);
     // the fused bias gradient needs a fixed quad per thread (256 %% (c/4) == 0) and 256 float4 of scratch (4*c >= 1024)
     SN_REQUIRE(!d->bias_grad || (256 % (d->c / 4) == 0 && d->c >= 256),

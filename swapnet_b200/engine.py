@@ -43,16 +43,23 @@ def _mix_seed(step_seed: int, stage_id: int) -> int:
 
 
 class Stage:
-    """conv -> [InstanceNorm] -> activation -> [dropout] (-> + residual), output written as operand
+    """conv -> [InstanceNorm | BatchNorm] -> activation -> [dropout] (-> + residual), output written as operand
     planes (and/or fp32).  `plain=True`: the conv output itself (after the epilogue activation) is
-    the stage output (head conv with tanh, PatchGAN logits)."""
+    the stage output (head conv with tanh, PatchGAN logits).
+
+    norm=True with `bn` (an nn.BatchNorm2d of the container): batch normalisation with bn's weight, bias and running
+    buffers, which the stage reads and updates in place.  The batch is `groups` consecutive groups of samples, each
+    normalised as a call of its own; Engine.training selects batch (train) or running (eval) statistics."""
 
     def __init__(self, eng: "Engine", name: str, kind: str, conv: nn.Module, x: Planes, *,
                  out: Optional[Planes] = None, norm: bool = False, act: int = ACT_NONE, slope: float = 0.2,
                  drop_p: float = 0.0, reflect_out: bool = False, residual: Optional[torch.Tensor] = None,
                  out_f32: Optional[torch.Tensor] = None, plain: bool = False, epi_act: int = ACT_NONE,
-                 need_dx: bool = True, y: Optional[torch.Tensor] = None, out_relu: Optional[Planes] = None):
+                 need_dx: bool = True, y: Optional[torch.Tensor] = None, out_relu: Optional[Planes] = None,
+                 bn: Optional[nn.BatchNorm2d] = None, groups: int = 1):
+        assert bn is None or norm, "a BatchNorm stage is a normalised stage"
         self.eng, self.name, self.kind = eng, name, kind
+        self.bn, self.groups = bn, groups
         self.id = len(eng.stages)
         eng.stages.append(self)
         dev = eng.device
@@ -94,22 +101,35 @@ class Stage:
         return self.n * self.oh * self.ow * ly.cout * ly.cin * k2
 
     # ---- forward ----
+    def _affine(self):
+        return (None, None) if self.bn is None else (self.bn.weight.data, self.bn.bias.data)
+
     def forward(self) -> None:
         self.layer.forward()
         if self.plain:
             return
-        if self.norm:
-            if getattr(self.layer, "fused_stats", False):
+        fused = getattr(self.layer, "fused_stats", False)
+        if self.bn is not None:
+            if not self.eng.training:
+                ops.bn_eval_stats(self.stats, self.n, self.cout, self.bn)
+            else:
+                if not fused:
+                    ops.plane_sums(self.y, self.cout, self.stats)
+                ops.bn_finalize(self.stats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn)
+        elif self.norm:
+            if fused:
                 ops.stats_finalize(self.stats, self.n * self.cout, self.oh * self.ow)
             else:
                 ops.plane_stats(self.y, self.cout, self.stats)
+        gamma, beta = self._affine()
         p = self.drop_p if self.eng.training else 0.0
         ops.norm_act_fwd(self.y, self.cout, self.stats, self.act, self.slope, p,
                          _mix_seed(self.eng.seed, self.id), residual=self.residual, out=self.out,
                          reflect_pad=self.reflect_out, out_f32=self.out_f32, drop_offset=self.drop_offset(),
-                         seed_dev=self.eng.seed_dev, stage_id=self.id)
+                         seed_dev=self.eng.seed_dev, stage_id=self.id, gamma=gamma, beta=beta)
         if self.out_relu is not None:
-            ops.norm_act_fwd(self.y, self.cout, self.stats, ACT_RELU, 0.0, 0.0, 0, out=self.out_relu)
+            ops.norm_act_fwd(self.y, self.cout, self.stats, ACT_RELU, 0.0, 0.0, 0, out=self.out_relu, gamma=gamma,
+                             beta=beta)
 
     # ---- backward ----
     def bind_backward(self, wgrad: bool = True) -> None:
@@ -141,10 +161,16 @@ class Stage:
             if wgrad and self.conv.bias is not None and self.conv.bias.grad is not None and ops.fused_bias_grad_ok(self.cout) \
                     and self.cout % 4 == 0 and getattr(self.layer, "bgrad_out", None) is not None:
                 bg = self.conv.bias.grad
+            bn = bn_grads = None
+            if self.bn is not None and not self.plain:
+                bn = self._affine()
+                if wgrad and self.bn.weight.grad is not None:
+                    bn_grads = (self.bn.weight.grad, self.bn.bias.grad)
             ops.norm_act_bwd(srcs, self.y, self.cout, None if self.plain else self.stats,
                              ACT_NONE if self.plain else self.act, self.dy, self.gstats, self.slope, p,
                              _mix_seed(self.eng.seed, self.id), drop_offset=self.drop_offset(),
-                             seed_dev=self.eng.seed_dev, stage_id=self.id, bias_grad=bg)
+                             seed_dev=self.eng.seed_dev, stage_id=self.id, bias_grad=bg, bn=bn, bn_groups=self.groups,
+                             bn_train=self.eng.training, bn_grads=bn_grads)
             if bg is not None:
                 self._layer_backward(wgrad, bias=False)
                 return
@@ -412,17 +438,19 @@ class WarpEngine(Engine):
 # PatchGAN
 # =============================================================================================
 class PatchGANEngine(Engine):
-    """NLayerDiscriminator on a [batch, S, S, pad64(input_nc)] operand (`self.din`)."""
+    """NLayerDiscriminator on a [batch, S, S, pad64(input_nc)] operand (`self.din`).  groups: the batch is that many
+    separate D calls stacked (the D step's fake and real halves), which matters to batch norm only."""
 
     def __init__(self, net: M.NLayerDiscriminator, batch: int, size: int, device, nsplit: int = 3,
-                 din: Optional[Planes] = None, input_grad: bool = False, train: bool = True):
+                 din: Optional[Planes] = None, input_grad: bool = False, train: bool = True, groups: int = 1):
         super().__init__(net, device, nsplit, train)
         B, S, dev = batch, size, self.device
         self.batch, self.size = B, S
         self.din = din if din is not None else self.planes(B, S, S, L.padc(net.input_nc))
         assert (self.din.n, self.din.h, self.din.w) == (B, S, S)
         convs = net.convs()
-        use_norm = net.norm == "instance"
+        bns = net.bns()
+        use_norm = net.norm != "none"
         x = self.din
         self.chain: List[Stage] = []
         h = S
@@ -431,7 +459,7 @@ class PatchGANEngine(Engine):
             oh = h // 2 if kind == "conv4s2" else h - 1
             out = self.planes(B, oh, oh, L.padc(conv.out_channels))
             st = Stage(self, f"model.{net.conv_index[i]}", kind, conv, x, out=out, norm=use_norm and i > 0,
-                       act=ACT_LRELU, slope=0.2, need_dx=(i > 0) or input_grad)
+                       act=ACT_LRELU, slope=0.2, need_dx=(i > 0) or input_grad, bn=bns[i], groups=groups)
             self.chain.append(st)
             x, h = out, oh
         self.last = Stage(self, f"model.{net.conv_index[-1]}", "conv4s1", convs[-1], x, plain=True)
@@ -461,7 +489,8 @@ class PatchGANEngine(Engine):
 # =============================================================================================
 class TextureEngine(Engine):
     """ROIAlign+repack -> encode (UNetDown 36->36) -> nearest upsample -> cat cloth -> pix2pix U-Net
-    (swapnet_modules.py:231-260, pix2pix_modules.py:113-262, norm = instance => bias on every conv).
+    (swapnet_modules.py:231-260, pix2pix_modules.py:113-262; the U-Net's [IN] below is its norm: instance (bias on
+    every conv), batch (BatchNorm2d, no bias but on U_0) or none (no bias but on U_0); `encode` is always IN).
 
     U-Net bookkeeping (depth j = 0 outermost .. nd-1 innermost; D_j / U_j = its down / up conv):
       L_{j+1} = leaky_relu([IN](D_j(.)))  is both the operand of D_{j+1} and, because the reference's
@@ -492,6 +521,7 @@ class TextureEngine(Engine):
                          act=ACT_LRELU, need_dx=False)
         chans = [blocks[j].down.out_channels for j in range(nd)]          # channels of x_{j+1}
         self.cu = [self.planes(B, S >> (j + 1), S >> (j + 1), 2 * chans[j]) for j in range(nd - 1)]
+        use_norm = unet.norm != "none"
         self.down: List[Stage] = []
         x = self.in_unet
         for j in range(nd):
@@ -502,8 +532,8 @@ class TextureEngine(Engine):
                 st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=False, act=ACT_RELU)
             else:
                 out = self.planes(B, h, h, L.padc(chans[j]))
-                st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=(j >= 1), act=ACT_LRELU,
-                        out_relu=self.cu[j].slice(0, chans[j]))
+                st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=(j >= 1) and use_norm, act=ACT_LRELU,
+                        out_relu=self.cu[j].slice(0, chans[j]), bn=blocks[j].down_bn)
             self.down.append(st)
             x = out
         self.up: List[Optional[Stage]] = [None] * nd
@@ -512,7 +542,7 @@ class TextureEngine(Engine):
             cout = blocks[j].up.out_channels
             drop = 0.5 if (blocks[j].use_dropout and not blocks[j].innermost) else 0.0
             self.up[j] = St(f"unet.U{j}", "convT4s2", blocks[j].up, src, out=self.cu[j - 1].slice(chans[j - 1], cout),
-                            norm=True, act=ACT_RELU, drop_p=drop)
+                            norm=use_norm, act=ACT_RELU, drop_p=drop, bn=blocks[j].up_bn)
         self.fakes = torch.zeros(B, S, S, self.ct, device=self.device)
         self.up[0] = St("unet.U0", "convT4s2", blocks[0].up, self.cu[0], plain=True, epi_act=ACT_TANH, y=self.fakes)
 

@@ -8,14 +8,14 @@ discriminators.py:45-88), GANLoss = vanilla BCE-with-logits with the reference's
 torch.optim.AdamW exactly as optimizers/__init__.py:37-60 builds it.
 
 What runs differently from the eager reference (results unchanged):
-  * D's fake and real passes of the D step run as ONE batch of 2B (InstanceNorm is per sample,
-    so this is exact) with per-half targets;
+  * D's fake and real passes of the D step run as ONE batch of 2B with per-half targets (InstanceNorm is per
+    sample; batch norm normalises each half with its own statistics and updates the running buffers fake first);
   * D's weight gradients are not computed in the G step (the reference computes and discards
     them, SURVEY App. B #5);
   * losses stay on the device until get_current_losses() is called.
 Unsupported option values raise (there is no eager fallback): --gan_mode other than vanilla,
---gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch,
---optimizer AdaBound.
+--gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch under data
+parallelism (no cross-rank batch statistics), --optimizer AdaBound.
 """
 from __future__ import annotations
 
@@ -120,6 +120,9 @@ class BaseGAN(BaseModel, ABC):
                                           "not provided")
             if opt.discriminator == "pixel":
                 raise NotImplementedError("--discriminator pixel is not provided on the B200 engines")
+            if opt.norm == "batch" and self._world > 1:
+                raise NotImplementedError("--norm batch under data parallelism: cross-rank batch statistics (SyncBN) "
+                                          "are not implemented; train on one GPU or use --norm instance / none")
             n_layers = 3 if opt.discriminator == "basic" else opt.n_layers_D
             self.net_discriminator = M.NLayerDiscriminator(self.get_D_inchannels(), 64, n_layers, opt.norm).to(self.device)
             M.init_weights(self.net_discriminator, opt.init_type, opt.init_gain)
@@ -216,7 +219,9 @@ class BaseGAN(BaseModel, ABC):
             g.bind_backward()
         if self.is_train and hasattr(self, "net_discriminator"):
             dn = self.net_discriminator
-            dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit)
+            # the D step's fake and real halves are two D calls: with batch norm, two sample groups with their own
+            # statistics and running-buffer updates (fake first)
+            dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit, groups=2)
             dd.alloc_grads()
             dd.bind_backward()
             dg = e["Dg"] = E.PatchGANEngine(dn, batch, size, self.device, self.nsplit,

@@ -142,7 +142,7 @@ class BaseModel(ABC):
         return self
 
     def eval(self):
-        """IN keeps no running stats, so eval only switches dropout off (SURVEY App. B #3)."""
+        """Dropout off (SURVEY App. B #3); with --norm batch the engines use the running statistics."""
         self.training = False
         for name in self.model_names:
             getattr(self, "net_" + name).eval()

@@ -79,28 +79,41 @@ class WarpModule(_NoEager):
         self.upsample_and_pad = _slots(nn.Conv2d(3 * 64, cloth_channels, 4, padding=1), 2, 4)
 
 
+NORMS = ("instance", "batch", "none")
+
+
+def check_norm(norm: str) -> str:
+    """modules/__init__.py:53-74 get_norm_layer's choices."""
+    if norm not in NORMS:
+        raise NotImplementedError(f"normalization layer [{norm}] is not found")
+    return norm
+
+
+def _norm_slot(norm: str, c: int) -> nn.Module:
+    """The module get_norm_layer(norm)(c) puts in a norm slot: a real BatchNorm2d (weight, bias and running buffers
+    under the reference's keys; initialised by init_weights in the same apply order), else a parameter-free
+    placeholder (InstanceNorm2d(affine=False) and Identity hold no state)."""
+    return nn.BatchNorm2d(c) if norm == "batch" else nn.Identity()
+
+
 class NLayerDiscriminator(_NoEager):
-    """PatchGAN 'basic' (n_layers=3).  norm: 'instance' (bias on every conv), 'none'."""
+    """PatchGAN 'basic' (n_layers=3).  norm: 'instance' (bias on every conv), 'batch' (BatchNorm2d at model.3/6/9,
+    no bias on the convs it follows), 'none'."""
 
     def __init__(self, input_nc, ndf=64, n_layers=3, norm="instance"):
         super().__init__()
-        if norm not in ("instance", "none"):
-            raise NotImplementedError(
-                f"--norm {norm}: only instance / none run on the B200 engine (batch norm couples samples "
-                "across the batch and is unsupported under data parallelism, SURVEY §8e)")
-        self.norm, self.input_nc, self.ndf, self.n_layers = norm, input_nc, ndf, n_layers
-        use_bias = norm == "instance"
-        per = 3 if norm == "instance" else 3  # conv, norm|identity, lrelu (get_norm_layer('none') -> Identity)
+        self.norm, self.input_nc, self.ndf, self.n_layers = check_norm(norm), input_nc, ndf, n_layers
+        use_bias = norm == "instance"    # discriminators.py:104-107
         seq = [nn.Conv2d(input_nc, ndf, 4, 2, 1), nn.Identity()]
         self.conv_index = [0]
         mult = 1
         for n in range(1, n_layers):
             prev, mult = mult, min(2 ** n, 8)
             self.conv_index.append(len(seq))
-            seq += [nn.Conv2d(ndf * prev, ndf * mult, 4, 2, 1, bias=use_bias)] + [nn.Identity()] * (per - 1)
+            seq += [nn.Conv2d(ndf * prev, ndf * mult, 4, 2, 1, bias=use_bias), _norm_slot(norm, ndf * mult), nn.Identity()]
         prev, mult = mult, min(2 ** n_layers, 8)
         self.conv_index.append(len(seq))
-        seq += [nn.Conv2d(ndf * prev, ndf * mult, 4, 1, 1, bias=use_bias)] + [nn.Identity()] * (per - 1)
+        seq += [nn.Conv2d(ndf * prev, ndf * mult, 4, 1, 1, bias=use_bias), _norm_slot(norm, ndf * mult), nn.Identity()]
         self.conv_index.append(len(seq))
         seq += [nn.Conv2d(ndf * mult, 1, 4, 1, 1)]
         self.model = nn.Sequential(*seq)
@@ -108,32 +121,55 @@ class NLayerDiscriminator(_NoEager):
     def convs(self):
         return [self.model[i] for i in self.conv_index]
 
+    def bns(self):
+        """The BatchNorm2d after each conv (None where there is none), aligned with convs()."""
+        return [self.model[i + 1] if isinstance(self.model[i + 1], nn.BatchNorm2d) else None
+                for i in self.conv_index[:-1]] + [None]
+
 
 class _SkipBlock(_NoEager):
     """pix2pix_modules.py:180-262 — Sequential positions of down conv / submodule / up conv differ per
     block type; reproduce the indices so the keys match (model.{i}.weight)."""
 
     def __init__(self, outer_nc, inner_nc, input_nc=None, submodule=None, outermost=False, innermost=False,
-                 use_dropout=False, use_bias=True):
+                 use_dropout=False, norm="instance"):
         super().__init__()
         self.outermost, self.innermost, self.use_dropout = outermost, innermost, use_dropout
+        use_bias = norm == "instance"    # pix2pix_modules.py:214-217
         input_nc = outer_nc if input_nc is None else input_nc
         down = nn.Conv2d(input_nc, inner_nc, 4, 2, 1, bias=use_bias)
+        self.down_bn_i = self.up_bn_i = None
         if outermost:      # [downconv, sub, uprelu, upconv, tanh]
             up = nn.ConvTranspose2d(inner_nc * 2, outer_nc, 4, 2, 1)
             seq = [down, submodule, nn.Identity(), up, nn.Identity()]
             self.down_i, self.sub_i, self.up_i = 0, 1, 3
         elif innermost:    # [downrelu, downconv, uprelu, upconv, upnorm]
             up = nn.ConvTranspose2d(inner_nc, outer_nc, 4, 2, 1, bias=use_bias)
-            seq = [nn.Identity(), down, nn.Identity(), up, nn.Identity()]
+            seq = [nn.Identity(), down, nn.Identity(), up, _norm_slot(norm, outer_nc)]
             self.down_i, self.sub_i, self.up_i = 1, None, 3
+            self.up_bn_i = 4
         else:              # [downrelu, downconv, downnorm, sub, uprelu, upconv, upnorm, (dropout)]
             up = nn.ConvTranspose2d(inner_nc * 2, outer_nc, 4, 2, 1, bias=use_bias)
-            seq = [nn.Identity(), down, nn.Identity(), submodule, nn.Identity(), up, nn.Identity()]
+            seq = [nn.Identity(), down, _norm_slot(norm, inner_nc), submodule, nn.Identity(), up,
+                   _norm_slot(norm, outer_nc)]
             if use_dropout:
                 seq.append(nn.Identity())
             self.down_i, self.sub_i, self.up_i = 1, 3, 5
+            self.down_bn_i, self.up_bn_i = 2, 6
         self.model = nn.Sequential(*seq)
+
+    def _bn(self, i):
+        return self.model[i] if i is not None and isinstance(self.model[i], nn.BatchNorm2d) else None
+
+    @property
+    def down_bn(self):
+        """BatchNorm2d after the down conv (norm 'batch', middle blocks), else None."""
+        return self._bn(self.down_bn_i)
+
+    @property
+    def up_bn(self):
+        """BatchNorm2d after the up conv (norm 'batch', all but the outermost block), else None."""
+        return self._bn(self.up_bn_i)
 
     @property
     def down(self):
@@ -149,15 +185,16 @@ class _SkipBlock(_NoEager):
 
 
 class UnetGenerator(_NoEager):
-    def __init__(self, input_nc, output_nc, num_downs, ngf=64, use_dropout=False, use_bias=True):
+    def __init__(self, input_nc, output_nc, num_downs, ngf=64, use_dropout=False, norm="instance"):
         super().__init__()
-        blk = _SkipBlock(ngf * 8, ngf * 8, innermost=True, use_bias=use_bias)
+        self.norm = check_norm(norm)
+        blk = _SkipBlock(ngf * 8, ngf * 8, innermost=True, norm=norm)
         for _ in range(num_downs - 5):
-            blk = _SkipBlock(ngf * 8, ngf * 8, submodule=blk, use_dropout=use_dropout, use_bias=use_bias)
-        blk = _SkipBlock(ngf * 4, ngf * 8, submodule=blk, use_bias=use_bias)
-        blk = _SkipBlock(ngf * 2, ngf * 4, submodule=blk, use_bias=use_bias)
-        blk = _SkipBlock(ngf, ngf * 2, submodule=blk, use_bias=use_bias)
-        self.model = _SkipBlock(output_nc, ngf, input_nc=input_nc, submodule=blk, outermost=True, use_bias=use_bias)
+            blk = _SkipBlock(ngf * 8, ngf * 8, submodule=blk, use_dropout=use_dropout, norm=norm)
+        blk = _SkipBlock(ngf * 4, ngf * 8, submodule=blk, norm=norm)
+        blk = _SkipBlock(ngf * 2, ngf * 4, submodule=blk, norm=norm)
+        blk = _SkipBlock(ngf, ngf * 2, submodule=blk, norm=norm)
+        self.model = _SkipBlock(output_nc, ngf, input_nc=input_nc, submodule=blk, outermost=True, norm=norm)
         self.num_downs = num_downs
 
     def blocks(self):
@@ -173,15 +210,14 @@ class TextureModule(_NoEager):
     def __init__(self, texture_channels=3, cloth_channels=19, num_roi=12, norm_type="instance", dropout=0.5,
                  img_size=128):
         super().__init__()
-        if norm_type not in ("instance",):
-            raise NotImplementedError(f"texture U-Net norm '{norm_type}': only instance runs on the B200 engine")
+        self.norm = check_norm(norm_type)     # the U-Net's norm; `encode` (a UNetDown) always uses InstanceNorm
         self.texture_channels, self.cloth_channels, self.num_roi = texture_channels, cloth_channels, num_roi
         self.img_size = img_size
         ch = texture_channels * num_roi
         self.encode = _down(ch, ch)
         num_downs = math.frexp(img_size)[1] - 1
         self.unet = UnetGenerator(ch + cloth_channels, texture_channels, num_downs,
-                                  use_dropout=dropout is not None, use_bias=True)
+                                  use_dropout=dropout is not None, norm=norm_type)
 
 
 def init_weights(net: nn.Module, init_type: str = "normal", init_gain: float = 0.02) -> None:
@@ -203,6 +239,9 @@ def init_weights(net: nn.Module, init_type: str = "normal", init_gain: float = 0
                 raise NotImplementedError(f"initialization method [{init_type}] is not implemented")
             if getattr(m, "bias", None) is not None:
                 init.constant_(m.bias.data, 0.0)
+        elif name.find("BatchNorm2d") != -1:
+            init.normal_(m.weight.data, 1.0, init_gain)
+            init.constant_(m.bias.data, 0.0)
 
     print("initialize network with %s" % init_type)
     net.apply(fn)

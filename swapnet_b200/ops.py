@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -530,14 +530,41 @@ def stats_finalize(stats: torch.Tensor, count: int, hw: int, eps: float = IN_EPS
     check(_lib.load().sn_stats_finalize(stats.data_ptr(), count, hw, eps, _stream()))
 
 
+def plane_sums(y: torch.Tensor, c: int, stats: torch.Tensor) -> None:
+    """y fp32 NHWC [n,h,w,pitch]; stats float64 [n, c, 2] <- (sum, sum of squares) over the plane."""
+    n, h, w, _ = y.shape
+    assert stats.dtype == torch.float64 and stats.numel() >= n * c * 2
+    check(_lib.load().sn_plane_sums(y.data_ptr(), _pitch(y), n, h * w, c, stats.data_ptr(), _stream()))
+
+
+def bn_finalize(stats: torch.Tensor, n: int, c: int, groups: int, hw: int, bn: "torch.nn.BatchNorm2d") -> None:
+    """Train-mode BatchNorm2d statistics: per-(n, c) (sum, sum of squares) -> (mean, rstd) of each sample's group, in
+    place; bn's running_mean / running_var / num_batches_tracked (device tensors) are updated group by group."""
+    assert stats.dtype == torch.float64 and n % groups == 0
+    assert bn.momentum is not None, "BatchNorm2d(momentum=None) (cumulative average) is not provided"
+    track = bn.track_running_stats
+    check(_lib.load().sn_bn_finalize(stats.data_ptr(), n, c, groups, hw, float(bn.eps), float(bn.momentum),
+                                     _ptr(bn.running_mean if track else None), _ptr(bn.running_var if track else None),
+                                     _ptr(bn.num_batches_tracked if track else None), _stream()))
+
+
+def bn_eval_stats(stats: torch.Tensor, n: int, c: int, bn: "torch.nn.BatchNorm2d") -> None:
+    """Eval-mode BatchNorm2d: stats [n, c, 2] <- (running_mean, rstd of running_var)."""
+    assert stats.dtype == torch.float64
+    check(_lib.load().sn_bn_eval_stats(stats.data_ptr(), n, c, bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                       float(bn.eps), _stream()))
+
+
 def norm_act_fwd(y: torch.Tensor, c: int, stats: Optional[torch.Tensor], act: int, slope: float = 0.2,
                  drop_p: float = 0.0, drop_seed: int = 0, residual: Optional[torch.Tensor] = None,
                  out: Optional[Planes] = None, reflect_pad: bool = False,
                  out_f32: Optional[torch.Tensor] = None, drop_offset: int = 0,
-                 seed_dev: Optional[torch.Tensor] = None, stage_id: int = 0) -> None:
+                 seed_dev: Optional[torch.Tensor] = None, stage_id: int = 0,
+                 gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None) -> None:
     """drop_offset: element offset of the keep-mask index (global sample index of the first local sample * h*w*c);
     seed_dev (uint64/int64[1] on the device) + stage_id: the per-stage seed is derived on the device from the
-    step seed stored there (CUDA-graph replay), drop_seed is then ignored."""
+    step seed stored there (CUDA-graph replay), drop_seed is then ignored.
+    gamma, beta (fp32 [c]): BatchNorm's affine, applied before the activation."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)
     d = SnNormActDesc()
@@ -562,6 +589,7 @@ def norm_act_fwd(y: torch.Tensor, c: int, stats: Optional[torch.Tensor], act: in
             d.out2_hi, d.out2_lo, d.out2_fmt = out.twin.hi.data_ptr(), out.twin.lo.data_ptr(), out.twin.fmt
     if out_f32 is not None:
         d.out_f32, d.f32_pitch = out_f32.data_ptr(), _pitch(out_f32)
+    d.gamma, d.beta = _ptr(gamma), _ptr(beta)
     check(_lib.load().sn_norm_act_fwd(C.byref(d), _stream()))
 
 
@@ -589,9 +617,13 @@ def _fill_srcs(arr, srcs: Sequence[GradSrc]) -> None:
 def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Optional[torch.Tensor], act: int,
                  dy: Planes, gstats: Optional[torch.Tensor] = None, slope: float = 0.2, drop_p: float = 0.0,
                  drop_seed: int = 0, drop_offset: int = 0, seed_dev: Optional[torch.Tensor] = None,
-                 stage_id: int = 0, bias_grad: Optional[torch.Tensor] = None) -> None:
+                 stage_id: int = 0, bias_grad: Optional[torch.Tensor] = None,
+                 bn: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, bn_groups: int = 1, bn_train: bool = True,
+                 bn_grads: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
     """bias_grad (fp32 [c], c in {256, 512, 1024}): += per-channel sums of the dy written — the bias gradient of the
-    conv that produced y — inside the apply pass (see fused_bias_grad_ok)."""
+    conv that produced y — inside the apply pass (see fused_bias_grad_ok).
+    bn = (gamma, beta): BatchNorm backward over `bn_groups` sample groups, with batch (bn_train) or running statistics
+    in `stats`; bn_grads = (d gamma, d beta) are accumulated (+=) when given."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)
     d = SnNormActBwdDesc()
@@ -608,6 +640,11 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
     d.dy_hi, d.dy_lo, d.dy_pitch, d.dy_coff = dy.hi.data_ptr(), dy.lo.data_ptr(), dy.pitch, dy.c_off
     d.dy_fmt = dy.fmt
     d.bias_grad = _ptr(bias_grad)
+    if bn is not None:
+        d.gamma, d.beta = bn[0].data_ptr(), bn[1].data_ptr()
+        d.bn_groups, d.bn_train = bn_groups, int(bn_train)
+        if bn_grads is not None:
+            d.gamma_grad, d.beta_grad = bn_grads[0].data_ptr(), bn_grads[1].data_ptr()
     check(_lib.load().sn_norm_act_bwd(C.byref(d), _stream()))
 
 
