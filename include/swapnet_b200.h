@@ -352,15 +352,12 @@ int sn_l1_loss_fwd_bwd(const float* a, int pitch, const float* b_nchw, int n, in
                        float weight, double* loss_acc, float* grad, int grad_pitch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * one-output-channel conv (PatchGAN logits, discriminators.py:131) as 1-tap GEMMs over a per-tap
+ * one-output-channel conv (PatchGAN logits, discriminators.py:131) over a per-tap
  * product image P[n,h,w,t] = sum_c x[n,h,w,c] W[0,c,t] (the input is read once instead of once per tap):
  *   y[n,oh,ow] = bias + sum_{kh,kw} P[n, oh+kh-pad, ow+kw-pad, kh*k+kw]
- *   dP[n,h,w,kh*k+kw] = dy[n, h-kh+pad, w-kw+pad]   (split planes; dy = split planes, channel 0)
  * ---------------------------------------------------------------------------------------- */
 int sn_tap_sum_fwd(const float* p, int p_pitch, int n, int h, int w, int k, int pad, const float* bias, float* y,
                    int y_pitch, void* stream);
-int sn_tap_shift_pack(const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int n, int h, int w, int k,
-                      int pad, void* dst_hi, void* dst_lo, int dst_pitch, int dst_coff, int fmt, void* stream);
 
 /* the one-output-channel conv on the CUDA cores at stream speed (csrc/patch_logits.cu; k = 4, stride 1):
  *   sn_to_one_fwd:   p[px][t] = sum_c x[px][c] * weight[c*16 + t]      x: split planes [npix][x_pitch], weight: the torch

@@ -160,7 +160,6 @@ SIGNATURES = {
     "sn_bce_logits_fwd_bwd": (_I, [_VP, _LL, _I, _F, _F, _F, _VP, _VP, _VP]),
     "sn_l1_loss_fwd_bwd": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _F, _VP, _VP, _I, _VP]),
     "sn_tap_sum_fwd": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _VP]),
-    "sn_tap_shift_pack": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_to_one_fwd": (_I, [_VP, _VP, _I, _I, _LL, _I, _VP, _I, _VP, _I, _VP]),
     "sn_to_one_wgrad": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP, _VP]),
     "sn_to_one_dgrad": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _I, _I, _VP, _I, _VP]),

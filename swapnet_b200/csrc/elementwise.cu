@@ -9,8 +9,6 @@
 //   models/texture_model.py:168-170 (L1).
 // All tensors are NHWC fp32 with an explicit pixel pitch; threads map to channels fastest
 // so that every warp touches contiguous 128-B lines.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "../../include/swapnet_b200.h"
 
@@ -1279,7 +1277,8 @@ __global__ void tap_gemm_simt_kernel(const SimtArgs a) {
 // 4-channel vectorised variants (C % 4 == 0, 16-B aligned fp32 rows, 8-B aligned plane rows).
 // One block = one image n and one slab of pixels, all channels; the per-channel statistics sit
 // in shared memory; threads walk the flattened (pixel, channel-quad) index so that a warp
-// touches 512 contiguous bytes.
+// touches 512 contiguous bytes.  The norm/activation kernels are compiled for 4 resident blocks
+// per SM (at most 64 registers): one quad in flight per thread, latency hidden by occupancy.
 // =================================================================================
 __device__ __forceinline__ void store_split4(uint16_t* hi, uint16_t* lo, long long off, const float v[4], int fmt) {
   uint16_t h[4], l[4];
@@ -1292,8 +1291,8 @@ __device__ __forceinline__ void store_split4(uint16_t* hi, uint16_t* lo, long lo
   if (lo) *reinterpret_cast<uint2*>(lo + off) = pl;
 }
 
-template <int MINB, bool AFF = false>
-__global__ void __launch_bounds__(256, MINB) norm_act_fwd_v4_kernel(const NormActFwdArgs a) {
+template <bool AFF>
+__global__ void __launch_bounds__(256, 4) norm_act_fwd_v4_kernel(const NormActFwdArgs a) {
   extern __shared__ float sm[];  // mean[C], rstd[C] (+ gamma[C], beta[C] when AFF)
   float* s_mean = sm;
   float* s_rstd = sm + a.C;
@@ -1446,8 +1445,8 @@ __device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned lon
 
 // grid (ceil(Q/bx), slabs, N), block (bx, 256/bx) with bx = min(32, pow2 >= Q): thread = channel quad,
 // strided over pixels (C = 64 layers — the largest tensors — use bx = 16, 16 pixel rows)
-template <int MINB, bool AFF = false>
-__global__ void __launch_bounds__(256, MINB) norm_act_bwd_reduce_v4_kernel(const NormActBwdArgs a) {
+template <bool AFF>
+__global__ void __launch_bounds__(256, 4) norm_act_bwd_reduce_v4_kernel(const NormActBwdArgs a) {
   __shared__ float red[256][8];
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1499,8 +1498,8 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_reduce_v4_kernel(const
   }
 }
 
-template <int MINB, bool AFF = false>
-__global__ void __launch_bounds__(256, MINB) norm_act_bwd_apply_v4_kernel(const NormActBwdArgs a) {
+template <bool AFF>
+__global__ void __launch_bounds__(256, 4) norm_act_bwd_apply_v4_kernel(const NormActBwdArgs a) {
   extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x C (+ gamma, beta when AFF)
   float* s_mean = sm;
   float* s_rstd = sm + a.C;
@@ -1560,278 +1559,6 @@ __global__ void __launch_bounds__(256, MINB) norm_act_bwd_apply_v4_kernel(const 
       atomicAdd(a.bias_grad + c + 2, t.z); atomicAdd(a.bias_grad + c + 3, t.w);
     }
   }
-}
-
-// ---------------------------------------------------------------------------------
-// U-way unrolled variants of the three kernels above (EXPERIMENT, off by default: see ew_use_v4): a thread issues the
-// loads of U channel quads (y, residual / every gradient source) BEFORE it computes and stores any of them.  The v4
-// kernels keep one quad in flight per thread, which at ~40 % occupancy leaves ~16-32 KB in flight per SM (ncu: 45-58 %
-// of the HBM copy rate).  Same arithmetic, same results bit for bit.
-// ---------------------------------------------------------------------------------
-struct QuadLoad {
-  float4 y;
-  float4 g[SN_MAX_SRC];
-};
-__device__ __forceinline__ void load_quad(const NormActBwdArgs& a, int n, int p, int c, QuadLoad& q) {
-  const int HW = a.H * a.W;
-  const long long pix = (long long)n * HW + p;
-  const int h = p / a.W, w = p - h * a.W;
-  q.y = *reinterpret_cast<const float4*>(a.y + pix * a.y_pitch + c);
-#pragma unroll
-  for (int i = 0; i < SN_MAX_SRC; ++i)
-    if (i < a.g.n) q.g[i] = gather_one4(a.g.s[i], n, h, w, a.H, a.W, c);
-}
-__device__ __forceinline__ void finish_quad(const NormActBwdArgs& a, unsigned long long seed, const QuadLoad& q, int n, int p,
-                                            int c, const float* mean, const float* rstd, float g[4], float xh[4]) {
-  const long long pix = (long long)n * a.H * a.W + p;
-  const float yy[4] = {q.y.x, q.y.y, q.y.z, q.y.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    xh[j] = (yy[j] - mean[j]) * rstd[j];
-    g[j] = 0.f;
-  }
-#pragma unroll
-  for (int i = 0; i < SN_MAX_SRC; ++i) {
-    if (i >= a.g.n) break;
-    const float gg[4] = {q.g[i].x, q.g[i].y, q.g[i].z, q.g[i].w};
-    const int act = a.g.s[i].act >= 0 ? a.g.s[i].act : a.act;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) g[j] += gg[j] * act_grad(xh[j], act, a.slope);
-  }
-  if (a.drop_thresh) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
-      g[j] = keep ? g[j] * a.drop_scale : 0.f;
-    }
-  }
-}
-
-template <int U>
-__global__ void __launch_bounds__(256, 2) norm_act_bwd_reduce_v4u_kernel(const NormActBwdArgs a) {
-  __shared__ float red[256][8];
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  const int c = q << 2;
-  const int n = blockIdx.z;
-  const int HW = a.H * a.W;
-  const int per = (HW + gridDim.y - 1) / gridDim.y;
-  const int p0 = blockIdx.y * per, p1 = min(HW, p0 + per);
-  float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-  if (c < a.C) {
-    float mean[4], rstd[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      mean[j] = (float)a.stats[((long long)n * a.C + c + j) * 2];
-      rstd[j] = (float)a.stats[((long long)n * a.C + c + j) * 2 + 1];
-    }
-    const int by = blockDim.y;
-    for (int pb = p0 + threadIdx.y; pb < p1; pb += U * by) {
-      QuadLoad ql[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-        if (pb + u * by < p1) load_quad(a, n, pb + u * by, c, ql[u]);
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if (pb + u * by >= p1) break;
-        float g[4], xh[4];
-        finish_quad(a, seed, ql[u], n, pb + u * by, c, mean, rstd, g, xh);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          s1[j] += g[j];
-          s2[j] += g[j] * xh[j];
-        }
-      }
-    }
-  }
-  const int slot = threadIdx.y * blockDim.x + threadIdx.x;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    red[slot][j] = s1[j];
-    red[slot][4 + j] = s2[j];
-  }
-  __syncthreads();
-  if (threadIdx.y == 0 && c < a.C) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      double u = 0.0, v = 0.0;
-      for (int r = 0; r < (int)blockDim.y; ++r) {
-        u += (double)red[r * blockDim.x + threadIdx.x][j];
-        v += (double)red[r * blockDim.x + threadIdx.x][4 + j];
-      }
-      atomic_add_f64(&a.gstats[((long long)n * a.C + c + j) * 2 + 0], u);
-      atomic_add_f64(&a.gstats[((long long)n * a.C + c + j) * 2 + 1], v);
-    }
-  }
-}
-
-template <int U>
-__global__ void __launch_bounds__(256, 2) norm_act_bwd_apply_v4u_kernel(const NormActBwdArgs a) {
-  extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x C
-  float* s_mean = sm;
-  float* s_rstd = sm + a.C;
-  float* s_m1 = sm + 2 * a.C;
-  float* s_m2 = sm + 3 * a.C;
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int n = blockIdx.y;
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    const long long k = ((long long)n * a.C + c) * 2;
-    s_mean[c] = a.stats ? (float)a.stats[k] : 0.f;
-    s_rstd[c] = a.stats ? (float)a.stats[k + 1] : 1.f;
-    s_m1[c] = a.stats ? (float)a.gstats[k] : 0.f;
-    s_m2[c] = a.stats ? (float)a.gstats[k + 1] : 0.f;
-  }
-  __syncthreads();
-  const int HW = a.H * a.W, Q = a.C >> 2;
-  const int per = (HW + gridDim.x - 1) / gridDim.x;
-  const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
-  const int bd = blockDim.x;
-  float bsum[4] = {0.f, 0.f, 0.f, 0.f};   // bias gradient: this thread's quad is fixed (blockDim % Q == 0)
-  for (int ib = threadIdx.x; ib < i1; ib += U * bd) {
-    QuadLoad ql[U];
-    int pp[U], cc[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int i = ib + u * bd;
-      const int pl = i / Q;
-      pp[u] = p0 + pl;
-      cc[u] = (i - pl * Q) << 2;
-      if (i < i1) load_quad(a, n, pp[u], cc[u], ql[u]);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (ib + u * bd >= i1) break;
-      const int c = cc[u];
-      float g[4], xh[4];
-      finish_quad(a, seed, ql[u], n, pp[u], c, s_mean + c, s_rstd + c, g, xh);
-      if (a.stats) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) g[j] = s_rstd[c + j] * (g[j] - s_m1[c + j] - xh[j] * s_m2[c + j]);
-      }
-      store_split4(a.hi, a.lo, ((long long)n * HW + pp[u]) * a.dy_pitch + a.dy_coff + c, g, a.fmt);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bsum[j] += g[j];
-    }
-  }
-  if (a.bias_grad) {   // host guarantees blockDim.x % Q == 0: thread t always handled quad t % Q
-    __syncthreads();
-    float4* red = reinterpret_cast<float4*>(sm);     // the statistics are no longer needed: 256 float4 fit in 4*C floats
-    red[threadIdx.x] = make_float4(bsum[0], bsum[1], bsum[2], bsum[3]);
-    __syncthreads();
-    if ((int)threadIdx.x < Q) {
-      float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int r = threadIdx.x; r < (int)blockDim.x; r += Q) {
-        const float4 v = red[r];
-        t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
-      }
-      const int c = threadIdx.x << 2;
-      atomicAdd(a.bias_grad + c, t.x); atomicAdd(a.bias_grad + c + 1, t.y);
-      atomicAdd(a.bias_grad + c + 2, t.z); atomicAdd(a.bias_grad + c + 3, t.w);
-    }
-  }
-}
-
-// forward: U quads of y (and of the residual) in flight per thread
-template <int U>
-__global__ void __launch_bounds__(256, 2) norm_act_fwd_v4u_kernel(const NormActFwdArgs a) {
-  extern __shared__ float sm[];  // mean[C], rstd[C]
-  float* s_mean = sm;
-  float* s_rstd = sm + a.C;
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int n = blockIdx.y;
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    s_mean[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2] : 0.f;
-    s_rstd[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2 + 1] : 1.f;
-  }
-  __syncthreads();
-  const int HW = a.H * a.W, Q = a.C >> 2;
-  const int per = (HW + gridDim.x - 1) / gridDim.x;
-  const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  const int i1 = (p1 - p0) * Q;
-  const int bd = blockDim.x;
-  for (int ib = threadIdx.x; ib < i1; ib += U * bd) {
-    float4 yv[U], rv[U];
-    int pp[U], cc[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int i = ib + u * bd;
-      const int pl = i / Q;
-      pp[u] = p0 + pl;
-      cc[u] = (i - pl * Q) << 2;
-      if (i < i1) {
-        const long long pix = (long long)n * HW + pp[u];
-        yv[u] = *reinterpret_cast<const float4*>(a.y + pix * a.y_pitch + cc[u]);
-        if (a.residual) rv[u] = *reinterpret_cast<const float4*>(a.residual + pix * a.res_pitch + cc[u]);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (ib + u * bd >= i1) break;
-      const int p = pp[u], c = cc[u];
-      const long long pix = (long long)n * HW + p;
-      float v[4] = {yv[u].x, yv[u].y, yv[u].z, yv[u].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float t = (v[j] - s_mean[c + j]) * s_rstd[c + j];
-        t = act_fwd(t, a.act, a.slope);
-        if (a.drop_thresh) {
-          const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
-          t = keep ? t * a.drop_scale : 0.f;
-        }
-        v[j] = t;
-      }
-      if (a.residual) {
-        v[0] += rv[u].x; v[1] += rv[u].y; v[2] += rv[u].z; v[3] += rv[u].w;
-      }
-      if (a.f32) *reinterpret_cast<float4*>(a.f32 + pix * a.f32_pitch + c) = make_float4(v[0], v[1], v[2], v[3]);
-      if (a.hi) {
-        if (!a.reflect) {
-          const long long off = pix * a.out_pitch + a.out_coff + c;
-          store_split4(a.hi, a.lo, off, v, a.fmt);
-          if (a.hi2) store_split4(a.hi2, a.lo2, off, v, a.fmt2);
-        } else {
-          const int hh = p / a.W, ww = p - hh * a.W;
-          const int Hp = a.H + 2, Wp = a.W + 2;
-          int rows[2], cols[2], nr = 1, nc = 1;
-          rows[0] = hh + 1;
-          cols[0] = ww + 1;
-          if (hh == 1) rows[nr++] = 0;
-          if (hh == a.H - 2) rows[nr++] = a.H + 1;
-          if (ww == 1) cols[nc++] = 0;
-          if (ww == a.W - 2) cols[nc++] = a.W + 1;
-          for (int ii = 0; ii < nr; ++ii)
-            for (int jj = 0; jj < nc; ++jj) {
-              const long long off = (((long long)n * Hp + rows[ii]) * Wp + cols[jj]) * a.out_pitch + a.out_coff + c;
-              store_split4(a.hi, a.lo, off, v, a.fmt);
-              if (a.hi2) store_split4(a.hi2, a.lo2, off, v, a.fmt2);
-            }
-        }
-      }
-    }
-  }
-}
-
-// measured (profiles/r02_*): the unrolled variants LOSE — 2 blocks / SM (112-126 registers) hide less latency than the
-// v4 kernels' 4 blocks with one quad in flight: bwd_apply 6.1 vs 4.4 ms per step, reduce 3.2 vs 2.2, forward 3.5 vs
-// 3.3.  They stay selectable (SN_EW_V4U=1) as the A/B evidence; the default is v4.
-// resident blocks per SM the v4 kernels are compiled for (register cap 64 / 51 / 42): SN_EW_MINB=4|5|6, A/B switch
-inline int ew_min_blocks() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SN_EW_MINB");
-    v = e ? atoi(e) : 4;
-    if (v != 5 && v != 6) v = 4;
-  }
-  return v;
-}
-inline bool ew_use_v4() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SN_EW_V4U");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
 }
 
 __global__ void sum_grads_v4_kernel(const GradSrcs g, int H, int W, int C, float* dst, int dst_pitch) {
@@ -2032,18 +1759,9 @@ int sn_fold_head_wgrad(const float* geff, int cout, int cin, float* dw, void* st
 
 int sn_plane_stats(const float* y, int pitch, int n, int hw, int c, float eps, double* stats,
                    void* stream) {
-  SN_REQUIRE(y && stats, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  SN_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * c, st));
-  const int cg = (c + 31) / 32;
-  int slabs = (SN_NUM_SMS * 4 + n * cg - 1) / (n * cg);
-  if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
-  if (slabs < 1) slabs = 1;
-  plane_stats_kernel<<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats);
-  LAUNCH_CHECK();
-  stats_finalize_kernel<<<(n * c + 255) / 256, 256, 0, st>>>(stats, n * c, hw, (double)eps);
-  LAUNCH_CHECK();
-  return SN_OK;
+  const int rc = sn_plane_sums(y, pitch, n, hw, c, stats, stream);
+  if (rc) return rc;
+  return sn_stats_finalize(stats, n * c, hw, eps, stream);
 }
 
 int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream) {
@@ -2119,17 +1837,10 @@ int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream) {
     // mean, rstd, gamma, beta in shared memory: 4 * c floats within the 48 KB a launch gets without opting in
     SN_REQUIRE(d->c <= 3072, "norm_act_fwd: the affine (BatchNorm) variant supports at most 3072 channels (c=%d)", d->c);
     dim3 grid(vslabs(d->h * d->w, d->n), d->n);
-    norm_act_fwd_v4_kernel<4, true><<<grid, 256, 4 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
+    norm_act_fwd_v4_kernel<true><<<grid, 256, 4 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
   } else if (vec) {
     dim3 grid(vslabs(d->h * d->w, d->n), d->n);
-    if (ew_use_v4()) {
-      const int mb = ew_min_blocks();
-      if (mb == 5) norm_act_fwd_v4_kernel<5><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
-      else if (mb == 6) norm_act_fwd_v4_kernel<6><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
-      else norm_act_fwd_v4_kernel<4><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
-    }
-    else
-      norm_act_fwd_v4u_kernel<4><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
+    norm_act_fwd_v4_kernel<false><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
   } else {
     dim3 blk = cblock(d->c);
     dim3 grid(slabs_for(d->h * d->w, d->n, blk.y), d->n);
@@ -2188,14 +1899,8 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       int slabs = (SN_NUM_SMS * 6 + d->n * qg - 1) / (d->n * qg);
       if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
       if (slabs < 1) slabs = 1;
-      if (aff) norm_act_bwd_reduce_v4_kernel<4, true><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
-      else if (ew_use_v4()) {
-        const int mb = ew_min_blocks();
-        if (mb == 5) norm_act_bwd_reduce_v4_kernel<5><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
-        else if (mb == 6) norm_act_bwd_reduce_v4_kernel<6><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
-        else norm_act_bwd_reduce_v4_kernel<4><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
-      }
-      else norm_act_bwd_reduce_v4u_kernel<2><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
+      if (aff) norm_act_bwd_reduce_v4_kernel<true><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
+      else norm_act_bwd_reduce_v4_kernel<false><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
     } else {
       const int cg = (d->c + 31) / 32;
       int slabs = (SN_NUM_SMS * 4 + d->n * cg - 1) / (d->n * cg);
@@ -2213,19 +1918,13 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
   }
   if (aff) {
     dim3 grid(vslabs(hw, d->n), d->n);
-    norm_act_bwd_apply_v4_kernel<4, true><<<grid, 256, 6 * d->c * sizeof(float), st>>>(a);
+    norm_act_bwd_apply_v4_kernel<true><<<grid, 256, 6 * d->c * sizeof(float), st>>>(a);
   } else if (vec) {
     dim3 grid(vslabs(hw, d->n), d->n);
     // the fused bias gradient needs a fixed quad per thread (256 %% (c/4) == 0) and 256 float4 of scratch (4*c >= 1024)
     SN_REQUIRE(!d->bias_grad || (256 % (d->c / 4) == 0 && d->c >= 256),
                "norm_act_bwd: fused bias gradient needs c in {256, 512, 1024} (c=%d)", d->c);
-    if (ew_use_v4()) {
-      const int mb = ew_min_blocks();
-      if (mb == 5) norm_act_bwd_apply_v4_kernel<5><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
-      else if (mb == 6) norm_act_bwd_apply_v4_kernel<6><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
-      else norm_act_bwd_apply_v4_kernel<4><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
-    }
-    else norm_act_bwd_apply_v4u_kernel<2><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
+    norm_act_bwd_apply_v4_kernel<false><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
   } else {
     SN_REQUIRE(!d->bias_grad, "norm_act_bwd: fused bias gradient is only available on the vectorised path");
     dim3 blk = cblock(d->c);

@@ -27,8 +27,6 @@
 // Warp roles (288 threads): warps 0..7 = two MMA warpgroups (64 rows of the
 // 128-row tile each; they also run the epilogue, registers -> global), warp 8 =
 // TMA producer.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "plan.h"
 
@@ -88,7 +86,7 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[C::kStages];
   __shared__ __align__(8) uint64_t empty_bar[C::kStages];
-  // dynamic tile schedule (p.tile_counter != null): the producer draws tile numbers from a device counter and hands them
+  // dynamic tile schedule: the producer draws tile numbers from a device counter (p.tile_counter) and hands them
   // to the MMA warps through a 4-deep ring, so a CTA that becomes resident late (SMs held by NCCL or by the
   // weight-gradient stream's CTAs) finds only the tiles nobody has taken yet instead of a fixed 1/gridDim share
   __shared__ __align__(8) uint64_t tr_full[kTileRing];
@@ -99,7 +97,6 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
   uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool dyn = p.tile_counter != nullptr;
 
   constexpr int cw = CW;                    // channels per A row: 64, 32 or 16
   constexpr int tps = 64 / cw;              // taps sharing one 64-deep stage (1, 2 or 4)
@@ -132,16 +129,13 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
       const uint32_t stage_tx = C::kPlanes * (p.a_rows * 128 + p.block_n * 128);
       uint32_t it = 0, tcount = 0;
       for (int tile = blockIdx.x;; ++tcount) {
-        int next = tile + (int)gridDim.x;
-        if (dyn) {
-          // the first tile is static; every further one a ticket.  The ticket for the NEXT tile is drawn now (its latency
-          // hides behind this tile's loads), the tile number goes to the other warps through the ring
-          if (tile < total_tiles) next = (int)gridDim.x + atomicAdd(p.tile_counter, 1);
-          const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
-          mbar_wait(&tr_empty[slot], rph ^ 1);
-          tile_ring[slot] = tile < total_tiles ? tile : -1;
-          mbar_arrive(&tr_full[slot]);
-        }
+        // the first tile is static; every further one a ticket.  The ticket for the NEXT tile is drawn now (its latency
+        // hides behind this tile's loads), the tile number goes to the other warps through the ring
+        const int next = tile < total_tiles ? (int)gridDim.x + atomicAdd(p.tile_counter, 1) : total_tiles;
+        const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
+        mbar_wait(&tr_empty[slot], rph ^ 1);
+        tile_ring[slot] = tile < total_tiles ? tile : -1;
+        mbar_arrive(&tr_full[slot]);
         if (tile >= total_tiles) break;
         int mt, nt, z;
         tile_coords(tile, mt, nt, z);
@@ -216,18 +210,14 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
     }
     const float oscale = p.b_scale ? p.b_scale[1] : 1.f;  // undo the power-of-two weight scale (exact)
     float acc[BN / 2];
-    uint32_t it = 0, tcount = 0;
-    for (int tile = blockIdx.x;; tile += gridDim.x, ++tcount) {
-      if (dyn) {
-        const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
-        mbar_wait(&tr_full[slot], rph);
-        tile = tile_ring[slot];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tr_empty[slot]);
-        if (tile < 0) break;
-      } else if (tile >= total_tiles) {
-        break;
-      }
+    uint32_t it = 0;
+    for (uint32_t tcount = 0;; ++tcount) {
+      const uint32_t slot = tcount % kTileRing, rph = (tcount / kTileRing) & 1;
+      mbar_wait(&tr_full[slot], rph);
+      const int tile = tile_ring[slot];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&tr_empty[slot]);
+      if (tile < 0) break;
       for (int k = 0; k < k_iters; ++k, ++it) {
         const uint32_t s = it % C::kStages;
         const uint32_t ph = (it / C::kStages) & 1;
@@ -353,7 +343,7 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
   }
 
   __syncthreads();
-  if (dyn && threadIdx.x == 0) {
+  if (threadIdx.x == 0) {
     // the last CTA to finish re-arms the counters for the next launch of this plan (every CTA's tickets are drawn
     // before it gets here; launches of one plan never overlap)
     __threadfence();
@@ -418,20 +408,13 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
       if (lane == 0) {
         const TapDesc xt = p.xtaps[tap_i];
         const uint32_t stage_tx = C::kPlanes * (2 * 8192 + y_blocks * y_block_bytes);
-        // rot_mode 0: every CTA walks the pixel tiles in the same order (a narrow wavefront shared through L2);
-        // 1: staggered per tap (blockIdx.y); 2: staggered per CTA
-        int rot = 0;
-        if (p.rot_mode == 1) rot = (int)(((long long)k_iters * blockIdx.y) / gridDim.y);
-        else if (p.rot_mode == 2)
-          rot = (int)(((long long)k_iters * ((blockIdx.x + blockIdx.y * gridDim.x) % p.sms)) / p.sms);
+        // every CTA walks the pixel tiles in the same order (a narrow wavefront shared through L2)
         for (int it = 0; it < k_iters; ++it) {
           const int s = it % C::kStages;
           const uint32_t ph = (it / C::kStages) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
           mbar_expect_tx(&full_bar[s], stage_tx);
-          int kr = it + rot;                       // per-CTA rotation of the pixel-tile order (see p.rot_mode)
-          if (kr >= k_iters) kr -= k_iters;
-          const int kt = kt0 + kr;
+          const int kt = kt0 + it;
           const int tw_i = kt % p.tiles_w;
           const int th_i = (kt / p.tiles_w) % p.tiles_h;
           const int tn_i = kt / (p.tiles_w * p.tiles_h);
@@ -756,32 +739,18 @@ int sn_tap_gemm_plan_init(TapGemmPlan* plan, const sn_tap_gemm_desc* d) {
     p.stats = d->stats;
   plan->stats_bytes = p.stats ? sizeof(double) * 2 * (size_t)d->m_n * d->n_valid : 0;
   p.tile_counter = nullptr;
-  {
-    static int dyn_ok = -1;
-    if (dyn_ok < 0) {
-      const char* e = getenv("SN_TAP_STATIC_TILES");   // A/B switch: the static tile striding of round 1
-      dyn_ok = (e && e[0] == '1') ? 0 : 1;
-    }
-    if (dyn_ok) {
-      SN_CHECK_CUDA(cudaMalloc(&p.tile_counter, 2 * sizeof(int)));
-      SN_CHECK_CUDA(cudaMemset(p.tile_counter, 0, 2 * sizeof(int)));
-    }
-  }
+  SN_CHECK_CUDA(cudaMalloc(&p.tile_counter, 2 * sizeof(int)));
+  SN_CHECK_CUDA(cudaMemset(p.tile_counter, 0, 2 * sizeof(int)));
   int rc;
   const void* a_pl[2] = {d->a_hi, d->a_lo};
   const void* b_pl[2] = {d->b_hi, d->b_lo};
-  static int merge_ok = -1;
-  if (merge_ok < 0) {
-    const char* e = getenv("SN_NO_MERGED_PLANES");   // A/B switch
-    merge_ok = (e && e[0] == '1') ? 0 : 1;
-  }
   const long long a_ps = d->nsplit == 3 ? (const char*)d->a_lo - (const char*)d->a_hi : 0;
   const long long b_ps = d->nsplit == 3 ? (const char*)d->b_lo - (const char*)d->b_hi : 0;
   // the lo tile must start on a swizzle-atom boundary (8 rows x 128 B)
-  p.a_merged = merge_ok && a_chunk == 64 && a_ps > 0 && a_ps % 16 == 0 && p.a_rows % 8 == 0;
+  p.a_merged = a_chunk == 64 && a_ps > 0 && a_ps % 16 == 0 && p.a_rows % 8 == 0;
   if (p.a_merged && d->a_parity)   // h parity moves into the channel coordinate of the merged parity map
     for (int t = 0; t < d->ntaps; ++t) p.taps[t].c_off += p.taps[t].hp * d->a_w * d->a_pitch;
-  p.b_merged = merge_ok && b_ps > 0 && b_ps % 16 == 0 && d->block_n % 8 == 0;
+  p.b_merged = b_ps > 0 && b_ps % 16 == 0 && d->block_n % 8 == 0;
   p.a_lo_off = p.a_merged ? p.a_rows * 128 : kTileBytes;
   p.b_lo_off = p.b_merged ? d->block_n * 128 : kTileBytes;
   for (int pl = 0; pl < (d->nsplit == 3 ? 2 : 1); ++pl) {
@@ -817,18 +786,15 @@ static int launch_tap(const TapGemmPlan* plan, cudaStream_t stream) {
   }
   // persistent launch: at most one CTA per SM; plan->grid = (M tiles, N tiles, phases)
   static int sms = 0;
-  static int one_tile_per_cta = -1;
   if (sms == 0) {
     int dev = 0;
     SN_CHECK_CUDA(cudaGetDevice(&dev));
     SN_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const char* e = getenv("SN_TAP_ONE_TILE_PER_CTA");   // A/B switch: the non-persistent schedule
-    one_tile_per_cta = (e && e[0] == '1') ? 1 : 0;
   }
   const int m_tiles = (int)plan->grid.x, n_tiles = (int)plan->grid.y;
   const int total = m_tiles * n_tiles * (int)plan->grid.z;
   if (plan->p.stats) SN_CHECK_CUDA(cudaMemsetAsync(plan->p.stats, 0, plan->stats_bytes, stream));
-  const int ctas = one_tile_per_cta ? total : (total < sms ? total : sms);
+  const int ctas = total < sms ? total : sms;
   tap_gemm_kernel<NSPLIT, CW, BN, F16>
       <<<ctas, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p, m_tiles, n_tiles, total);
   SN_CHECK_CUDA(cudaGetLastError());
@@ -924,12 +890,10 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   const void* x_pl[2] = {d->x_hi, d->x_lo};
   const void* y_pl[2] = {d->y_hi, d->y_lo};
   {
-    const char* e = getenv("SN_NO_MERGED_PLANES");
-    const bool merge_ok = !(e && e[0] == '1');
     const long long x_ps = d->nsplit == 3 ? (const char*)d->x_lo - (const char*)d->x_hi : 0;
     const long long y_ps = d->nsplit == 3 ? (const char*)d->y_lo - (const char*)d->y_hi : 0;
-    p.x_merged = merge_ok && x_ps > 0 && x_ps % 16 == 0 && tw * th * nb == 64;
-    p.y_merged = merge_ok && y_ps > 0 && y_ps % 16 == 0 && tw * th * nb == 64 && y_chunk == 64 && d->ngroups == 0;
+    p.x_merged = x_ps > 0 && x_ps % 16 == 0 && tw * th * nb == 64;
+    p.y_merged = y_ps > 0 && y_ps % 16 == 0 && tw * th * nb == 64 && y_chunk == 64 && d->ngroups == 0;
     for (int t = 0; t < d->ntaps; ++t) {   // h parity -> channel coordinate of the merged parity maps
       if (p.x_merged && d->x_parity) p.xtaps[t].c_off += p.xtaps[t].hp * d->x_w * d->x_pitch;
       if (p.y_merged && d->y_parity) p.ytaps[t].c_off += p.ytaps[t].hp * d->y_w * d->y_pitch;
@@ -952,13 +916,7 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   plan->nsplit = d->nsplit;
   const int base_ctas = p.m_tiles * p.n_tiles * grid_y;
   const int total = p.tiles_w * p.tiles_h * p.tiles_n;
-  p.rot_mode = 0;
-  p.sms = sm_count;
-  if (const char* e = getenv("SN_WGRAD_ROT")) p.rot_mode = atoi(e);
   int ks = d->ksplit;
-  if (const char* e = getenv("SN_WGRAD_KSPLIT")) {   // experiment override
-    if (atoi(e) > 0) ks = atoi(e);
-  }
   if (ks <= 0) {  // aim for ~3 waves, at least 8 k-iterations per CTA
     ks = (3 * sm_count + base_ctas - 1) / base_ctas;
     int max_ks = total / 8;

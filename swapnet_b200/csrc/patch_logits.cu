@@ -10,7 +10,6 @@
 //   dW[0,c,t] = sum_px x[px, c] dP[px, t]                  (to_one_wgrad_kernel)
 //   dx[px, c] = sum_t dP[px, t] W[0, c, t]                 (to_one_dgrad_kernel)
 // x arrives as fp16-split planes (hi + lo = 22 mantissa bits), products and sums are fp32 FMAs.
-// (tap_shift_pack + the 1-tap tensor-core GEMMs of round 1 remain for the A/B switch SN_TO_ONE_TC=1.)
 #include "common.cuh"
 #include "../../include/swapnet_b200.h"
 
@@ -45,33 +44,6 @@ __global__ void tap_sum_fwd_kernel(const float* __restrict__ P, int ppitch, int 
       }
     }
     y[i * ypitch] = acc + (bias ? bias[0] : 0.f);
-  }
-}
-
-// dP[n,h,w,t] = dy[n, h - kh + pad, w - kw + pad] (0 outside); dy given as split planes (channel 0)
-__global__ void tap_shift_pack_kernel(const uint16_t* __restrict__ dy_hi, const uint16_t* __restrict__ dy_lo,
-                                      int dypitch, int dyfmt, int N, int H, int W, int K, int pad,
-                                      uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, int pitch, int coff,
-                                      int fmt) {
-  const int OH = H + 2 * pad - K + 1, OW = W + 2 * pad - K + 1;
-  const long long total = (long long)N * H * W;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int w = (int)(i % W), h = (int)((i / W) % H);
-    const long long n = i / ((long long)W * H);
-    for (int kh = 0; kh < K; ++kh)
-      for (int kw = 0; kw < K; ++kw) {
-        const int oh = h - kh + pad, ow = w - kw + pad;
-        float v = 0.f;
-        if (oh >= 0 && oh < OH && ow >= 0 && ow < OW) {
-          const long long o = ((n * OH + oh) * OW + ow) * dypitch;
-          v = decode16(dy_hi[o], dyfmt) + (dy_lo ? decode16(dy_lo[o], dyfmt) : 0.f);
-        }
-        uint16_t a, b;
-        split16(v, fmt, a, b);
-        hi[i * pitch + coff + kh * K + kw] = a;
-        lo[i * pitch + coff + kh * K + kw] = b;
-      }
   }
 }
 
@@ -274,16 +246,6 @@ int sn_tap_sum_fwd(const float* p, int p_pitch, int n, int h, int w, int k, int 
   const long long total = (long long)n * (h + 2 * pad - k + 1) * (w + 2 * pad - k + 1);
   tap_sum_fwd_kernel<<<grid_for(total), kThreads, 0, (cudaStream_t)stream>>>(p, p_pitch, n, h, w, k, pad, bias, y,
                                                                              y_pitch);
-  LAUNCH_CHECK();
-  return SN_OK;
-}
-
-int sn_tap_shift_pack(const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int n, int h, int w, int k,
-                      int pad, void* dst_hi, void* dst_lo, int dst_pitch, int dst_coff, int fmt, void* stream) {
-  SN_REQUIRE(dy_hi && dst_hi && dst_lo && k >= 1 && k * k <= dst_pitch - dst_coff, "tap_shift_pack: bad arguments");
-  tap_shift_pack_kernel<<<grid_for((long long)n * h * w), kThreads, 0, (cudaStream_t)stream>>>(
-      (const uint16_t*)dy_hi, (const uint16_t*)dy_lo, dy_pitch, dy_fmt, n, h, w, k, pad, (uint16_t*)dst_hi,
-      (uint16_t*)dst_lo, dst_pitch, dst_coff, fmt);
   LAUNCH_CHECK();
   return SN_OK;
 }

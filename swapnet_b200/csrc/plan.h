@@ -36,7 +36,7 @@ struct alignas(64) TapGemmParams {
   int a_lo_off, b_lo_off;   // byte offset of the lo tile behind the hi tile inside a stage
   int stack_slot, stack_c;  // > 0: N = 4 output-parity phases side by side (sn_tap_gemm_desc.stack_slot)
   double* stats;            // non-null: accumulate per-(image, channel) sum / sum of squares of the output (fused IN stats)
-  int* tile_counter;        // non-null: dynamic tile schedule — [0] next ticket, [1] CTAs finished (self-resetting)
+  int* tile_counter;        // dynamic tile schedule: [0] next ticket, [1] CTAs finished (self-resetting)
 };
 
 struct alignas(64) WgradParams {
@@ -56,8 +56,6 @@ struct alignas(64) WgradParams {
   int y_chunk;  // 64 / 32 / 16 channels per Y row
   int ngroups;  // > 0: narrow-Y tap groups (grid.y = group)
   int x_merged, y_merged;   // hi+lo of a 64-channel block in one TMA box (see TapGemmParams)
-  int rot_mode; // pixel-tile order stagger (0 none, 1 per tap, 2 per CTA)
-  int sms;      // SMs of the device (rot_mode 2)
   short gstart[SN_MAX_TAPS], gsize[SN_MAX_TAPS];
 };
 

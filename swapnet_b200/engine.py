@@ -28,14 +28,8 @@ from torch import nn
 from . import lowering as L
 from . import modules as M
 from . import ops
-import os
-
 from .layers import ConvLayer, ToOneConvLayer
 from .ops import ACT_LRELU, ACT_NONE, ACT_RELU, ACT_TANH, FMT_BF16, GradSrc, Planes
-
-
-TO_ONE = os.environ.get("SN_NO_TO_ONE", "0") != "1"    # A/B switch for layers.ToOneConvLayer
-WGRAD_OVERLAP = os.environ.get("SN_NO_WGRAD_OVERLAP", "0") != "1"   # A/B switch: weight gradients on a second stream
 
 
 def _mix_seed(step_seed: int, stage_id: int) -> int:
@@ -65,7 +59,7 @@ class Stage:
         dev = eng.device
         # a stride-1 conv with ONE output channel (the PatchGAN logits) runs as 1-tap GEMMs (layers.ToOneConvLayer)
         to_one = (kind == "conv4s1" and conv.out_channels == 1 and epi_act == ACT_NONE and conv.in_channels % 8 == 0
-                  and conv.in_channels <= 1024 and x.c_off % 8 == 0 and TO_ONE)
+                  and conv.in_channels <= 1024 and x.c_off % 8 == 0)
         self.layer = (ToOneConvLayer if to_one else ConvLayer)(
             kind, conv.weight.data, None if conv.bias is None else conv.bias.data, x, nsplit=eng.nsplit, act=epi_act,
             name=name)
@@ -211,8 +205,8 @@ class Engine:
         self.flat_grad: Optional[torch.Tensor] = None
 
     def wgrad_stream(self) -> Optional[torch.cuda.Stream]:
-        """Second stream for the weight-gradient GEMMs (None: launch in line — A/B switch, per-launch tracing)."""
-        if not WGRAD_OVERLAP or ops.Plan.trace is not None:
+        """Second stream for the weight-gradient GEMMs (None: launch in line, for per-launch tracing)."""
+        if ops.Plan.trace is not None:
             return None
         if self._wgrad_stream is None:
             self._wgrad_stream = torch.cuda.Stream(device=self.device)
@@ -256,11 +250,7 @@ class Engine:
 
     def pack(self) -> None:
         """Kernel-layout copies of the (updated) torch weights: one scale launch + one pack launch for the whole
-        network (ops.PackTable), plus the head's effective-tap packs.  SN_PACK_PER_LAYER=1: the per-layer launches."""
-        if os.environ.get("SN_PACK_PER_LAYER", "0") == "1":
-            for s in self.stages:
-                s.layer.pack()
-            return
+        network (ops.PackTable), plus the head's effective-tap packs."""
         if self._pack_table is None:
             self._pack_table = ops.PackTable(self.device)
             self._pack_extra = [s.layer for s in self.stages if s.layer.register_packs(self._pack_table)]

@@ -16,10 +16,6 @@ from . import lowering as L
 from . import ops
 from .ops import ACT_NONE, PackedWeights, Planes
 
-import os
-
-HEAD_STACKED = os.environ.get("SN_HEAD_STACKED", "1") != "0"   # A/B switch: the head forward as one 9-tap GEMM
-
 
 class ConvLayer:
     def __init__(self, kind: str, weight: torch.Tensor, bias: Optional[torch.Tensor], x: Planes, *,
@@ -43,7 +39,7 @@ class ConvLayer:
         self.block_n = L.pick_block_n(self.cout)
         self.t = L.ntaps(kind)
         self.wscale = torch.ones(2, dtype=torch.float32, device=dev)  # (s, 1/s), shared by fwd and dgrad packs
-        self.stacked = kind == "head" and HEAD_STACKED and self.cout <= L.HEAD_SLOT and self.k_pad % 64 == 0
+        self.stacked = kind == "head" and self.cout <= L.HEAD_SLOT and self.k_pad % 64 == 0
         if self.stacked:
             self.rows_pad = 4 * L.HEAD_SLOT
             self.wp = PackedWeights(self.rows_pad, 9 * self.k_pad, dev, self.wscale)
@@ -81,7 +77,7 @@ class ConvLayer:
         self.y = y
         self.fwd_plans = []
         self.fused_stats = False
-        if os.environ.get("SN_NO_FUSED_STATS", "0") == "1" or y_c_off != 0 or self.act != ACT_NONE:
+        if y_c_off != 0 or self.act != ACT_NONE:
             stats = None
         if self.stacked:
             d = ops.tap_gemm_desc(self.x, L.head_stacked_spec(self.in_h, self.in_w), self.wp, self.k_pad, y,

@@ -24,7 +24,6 @@ from argparse import ArgumentParser
 from typing import Optional
 
 import gc
-import os
 
 import torch
 
@@ -143,7 +142,7 @@ class BaseGAN(BaseModel, ABC):
             self._sp_ready = False          # True inside optimize_parameters(): labels were drawn by the step prologue
             self._graphs = {}               # (batch, size, training, input signature) -> captured step
             self._eager_steps = {}
-            self.graph_enabled = os.environ.get("SN_NO_GRAPH", "0") != "1" and bool(getattr(opt, "b200_graph", 1))
+            self.graph_enabled = bool(getattr(opt, "b200_graph", 1))
             self._acc_host = None                       # host copy of _acc for the current step (one D2H per step)
             lam = float(opt.lambda_gan)
             self.loss_D_fake = LazyLoss(lambda: self.loss_values()[0])

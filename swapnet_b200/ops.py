@@ -898,27 +898,11 @@ def gram_bwd(m: torch.Tensor, x: torch.Tensor, nhwc: bool, dx: torch.Tensor, acc
 # ---------------------------------------------------------------------------------------------
 # one-output-channel conv helpers (csrc/patch_logits.cu)
 # ---------------------------------------------------------------------------------------------
-def pack_weights_raw(weight: torch.Tensor, s_row: int, s_k: int, rows: int, k_real: int, k_pad: int,
-                     dst: PackedWeights) -> None:
-    """dst[r][k] = split(weight.flat[r*s_row + k*s_k]) for k < k_real (single tap), zero up to k_pad."""
-    assert weight.is_contiguous() and weight.dtype == torch.float32 and dst.rows >= rows and dst.k_total == k_pad
-    slots = (C.c_int * 1)(0)
-    check(_lib.load().sn_pack_weights(weight.data_ptr(), s_row, s_k, rows, 1, 1, slots, k_real, k_pad, dst.hi.data_ptr(),
-                                      dst.lo.data_ptr(), dst.fmt, None if dst.scale is None else dst.scale.data_ptr(),
-                                      _stream()))
-
-
 def tap_sum_fwd(p: torch.Tensor, k: int, pad: int, bias: Optional[torch.Tensor], y: torch.Tensor) -> None:
     n, h, w, _ = p.shape
     assert y.shape[:3] == (n, h + 2 * pad - k + 1, w + 2 * pad - k + 1)
     check(_lib.load().sn_tap_sum_fwd(p.data_ptr(), _pitch(p), n, h, w, k, pad, _ptr(bias), y.data_ptr(), _pitch(y),
                                      _stream()))
-
-
-def tap_shift_pack(dy: Planes, k: int, pad: int, dst: Planes) -> None:
-    assert (dy.n, dy.h, dy.w) == (dst.n, dst.h + 2 * pad - k + 1, dst.w + 2 * pad - k + 1) and dst.c >= k * k
-    check(_lib.load().sn_tap_shift_pack(dy.hi_ptr, dy.lo_ptr, dy.pitch, dy.fmt, dst.n, dst.h, dst.w, k, pad,
-                                        dst.hi.data_ptr(), dst.lo.data_ptr(), dst.pitch, dst.c_off, dst.fmt, _stream()))
 
 
 def to_one_fwd(x: Planes, weight: torch.Tensor, p: torch.Tensor) -> None:

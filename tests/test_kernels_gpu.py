@@ -65,6 +65,7 @@ CONV_CASES = [
     ("conv4s1", 1, 64, 64, 8, 8),
     ("head", 2, 192, 19, 32, 32),
     ("head", 1, 64, 19, 16, 48),
+    ("head", 2, 192, 27, 16, 16),        # more outputs than HEAD_SLOT: the unstacked 4-phase forward
     ("conv4s2", 2, 19, 64, 32, 32),      # 19 -> 32-channel rows (SWIZZLE_64B)
     ("conv4s1", 2, 16, 32, 16, 16),      # exactly 16 channels (SWIZZLE_32B), narrow dy too
     ("convT4s2", 2, 32, 16, 8, 8),

@@ -152,7 +152,7 @@ def test_to_one_factorisation():
                     iw = ow + kw - 1
                     if 0 <= iw < w:
                         out[:, oh, ow] += P[:, ih, iw, t]          # sn_tap_sum_fwd
-                        dP[:, ih, iw, t] = GY[:, oh, ow]           # sn_tap_shift_pack
+                        dP[:, ih, iw, t] = GY[:, oh, ow]           # dP = dy shifted by tap t
     torch.testing.assert_close(out + b, y.detach()[:, 0], rtol=1e-12, atol=1e-12)
     dW = torch.einsum("nhwc,nhwt->ct", X, dP).reshape(1, cin, 4, 4)
     dX = dP @ Wt.t()
