@@ -73,6 +73,18 @@ CONV_CASES = [
     ("conv3z", 2, 64, 64, 32, 48),
     ("conv3z", 1, 128, 256, 16, 16),
     ("conv3z", 3, 256, 256, 4, 4),
+    # the warp engine at S = 192: planes 96/48/24/12/6/3 wide, PatchGAN 23x23 (conv: 27-row tiles of 3 whole 3x3
+    # images, a_rows % 8 != 0 -> unmerged A; weight gradient: 4x4 patches of 4 images over a 3x3 plane, masked)
+    ("conv4s2", 2, 64, 128, 24, 24),
+    ("conv4s2", 3, 128, 256, 6, 6),
+    ("convT4s2", 3, 256, 128, 3, 3),
+    ("conv3r", 2, 128, 128, 12, 12),
+    ("conv4s1", 2, 256, 512, 24, 24),
+    ("head", 2, 64, 19, 48, 48),
+    # texture-stage widths: encode 36 -> 36, the U-Net's first conv 36 + 19 = 55 -> 64, the decoder's 36-channel output
+    ("conv4s2", 2, 36, 36, 64, 64),
+    ("conv4s2", 2, 55, 64, 64, 64),
+    ("convT4s2", 2, 128, 36, 16, 16),
 ]
 
 
@@ -160,7 +172,10 @@ def test_conv_backward(kind, n, cin, cout, h, w):
         gx, gw, gb = torch.autograd.grad(yr, (xr, wr, br), gy.double())
     dyc = L.padc(cout) if layer.x.c >= 64 else L.pad64(cout)   # one wgrad operand must carry >= 64 channels
     dy = ops.Planes(n, oh, ow, dyc, dev(), fmt=ops.FMT_BF16)  # gradients travel as bf16-split
-    ops.pack_planes(gy.to(dev()), dy)
+    if cout * 33 * 4 > 48 * 1024:   # the NCHW packer stages [c][33] floats in shared memory: wide gradients go NHWC
+        ops.pack_planes(nhwc(gy).to(dev()), dy, nhwc=True)
+    else:
+        ops.pack_planes(gy.to(dev()), dy)
     ih, iw = (h + 2, w + 2) if kind == "conv3r" else (h, w)
     dx = torch.full((n, ih, iw, cin + 3), 5.0, device=dev())
     wg = torch.zeros_like(layer.weight)
@@ -688,7 +703,9 @@ def test_to_one_conv_layer(n, cin, h, w):
 
 @pytest.mark.parametrize("kind,n,cin,cout,h,w,fused", [("conv4s2", 2, 64, 128, 32, 64, True), ("convT4s2", 2, 128, 64, 16, 16, True),
                                                      ("conv3r", 3, 128, 128, 32, 32, True), ("conv4s1", 2, 128, 256, 64, 64, True),
-                                                     ("conv4s2", 3, 128, 192, 16, 16, False)])
+                                                     ("conv4s2", 3, 128, 192, 16, 16, False),
+                                                     ("conv4s2", 2, 36, 36, 64, 64, False),   # n_valid % 16 != 0
+                                                     ("conv4s2", 2, 55, 64, 64, 64, True)])
 def test_fused_instance_norm_statistics(kind, n, cin, cout, h, w, fused):
     """InstanceNorm statistics accumulated by the GEMM epilogue (sn_tap_gemm_desc.stats + sn_stats_finalize) equal the
     per-(image, channel) mean and 1/sqrt(biased variance + eps) of the conv output; planes smaller than a tile (several
