@@ -347,6 +347,16 @@ int sn_bce_logits_fwd_bwd(const float* pred, long long count_per_half, int halve
 /* targets read from device memory: t_dev[0] (first half) and t_dev[1] (second half) */
 int sn_bce_logits_fwd_bwd_dev(const float* pred, long long count_per_half, int halves, const float* t_dev,
                               float gscale, double* loss_acc, float* dpred, void* stream);
+/* GANLoss objectives (loss.py:53-62,110-130), the --gan_mode values that need no gradient penalty. */
+enum { SN_GAN_BCE = 0, SN_GAN_MSE = 1, SN_GAN_WGAN = 2 };
+/* One GAN objective over `halves` (1 or 2) consecutive blocks of count_per_half predictions, each with its own scalar:
+ * loss_acc[half] += the unweighted batch mean, dpred = gscale * d(mean)/d(pred) (dpred may be null).
+ *   SN_GAN_BCE   vanilla: BCEWithLogitsLoss(pred, t)     t = t_dev[half] if t_dev is non-null, else t0 / t1
+ *   SN_GAN_MSE   lsgan:   MSELoss(pred, t)               t as for SN_GAN_BCE
+ *   SN_GAN_WGAN  wgan:    t * mean(pred), t0 / t1 = +1 (fake) or -1 (real); t_dev must be null
+ * SN_GAN_BCE runs the kernel of sn_bce_logits_fwd_bwd(_dev). */
+int sn_gan_loss_fwd_bwd_dev(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
+                            const float* t_dev, float gscale, double* loss_acc, float* dpred, void* stream);
 /* L1Loss(a, b) * weight (texture_model.py:168-170); a NHWC (pitch), b NCHW; grad wrt a. */
 int sn_l1_loss_fwd_bwd(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c,
                        float weight, double* loss_acc, float* grad, int grad_pitch, void* stream);

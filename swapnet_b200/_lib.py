@@ -158,6 +158,7 @@ SIGNATURES = {
     "sn_ce_loss_fwd_bwd": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _I, _F, _VP, _VP, _I, _VP]),
     "sn_ce_tanh_bwd": (_I, [_VP, _I, _VP, _I, C.POINTER(SnGradSrc), _I, _I, _I, _I, _I, _F, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "sn_bce_logits_fwd_bwd": (_I, [_VP, _LL, _I, _F, _F, _F, _VP, _VP, _VP]),
+    "sn_gan_loss_fwd_bwd_dev": (_I, [_I, _VP, _LL, _I, _F, _F, _VP, _F, _VP, _VP, _VP]),
     "sn_l1_loss_fwd_bwd": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _F, _VP, _VP, _I, _VP]),
     "sn_tap_sum_fwd": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _VP]),
     "sn_to_one_fwd": (_I, [_VP, _VP, _I, _I, _LL, _I, _VP, _I, _VP, _I, _VP]),

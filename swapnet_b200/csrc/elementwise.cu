@@ -1171,9 +1171,16 @@ __global__ void __launch_bounds__(128) ce_tanh_bwd_kernel(const float* __restric
   block_add_double(local * (double)weight / (double)npix, loss_acc);
 }
 
-__global__ void bce_logits_kernel(const float* __restrict__ pred, long long count, int halves, float t0,
-                                  float t1, const float* __restrict__ t_dev, float gscale, double* loss_acc,
-                                  float* __restrict__ dpred) {
+// GANLoss (loss.py:110-130) over `halves` consecutive blocks of `count` predictions, one per blockIdx.y, each with its own
+// scalar t (t_dev[half] when t_dev is set, else t0 / t1): loss_acc[half] += the objective's batch mean, and
+// dpred = gscale * d(mean)/dx in the same pass.
+//   SN_GAN_BCE   BCEWithLogitsLoss(x, t)      dL/dx = (sigmoid(x) - t) / count
+//   SN_GAN_MSE   MSELoss(x, t)                dL/dx = 2 (x - t) / count
+//   SN_GAN_WGAN  t * mean(x), t = +1 / -1     dL/dx = t / count            (t is a sign, not a label)
+template <int OBJ>
+__global__ void gan_loss_kernel(const float* __restrict__ pred, long long count, int halves, float t0, float t1,
+                                const float* __restrict__ t_dev, float gscale, double* loss_acc,
+                                float* __restrict__ dpred) {
   const int half = blockIdx.y;
   const float t = t_dev ? t_dev[half] : (half == 0 ? t0 : t1);
   double local = 0.0;
@@ -1181,13 +1188,23 @@ __global__ void bce_logits_kernel(const float* __restrict__ pred, long long coun
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count;
        i += (long long)gridDim.x * blockDim.x) {
     const float x = pred[half * count + i];
-    // max(x,0) - x*t + log1p(exp(-|x|))   (ATen binary_cross_entropy_with_logits)
-    const float l = (1.f - t) * x + (fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x))));
-    local += (double)l;
-    const float sg = 1.f / (1.f + expf(-x));
-    if (dpred) dpred[half * count + i] = gs * (sg - t);
+    if constexpr (OBJ == SN_GAN_BCE) {
+      // max(x,0) - x*t + log1p(exp(-|x|))   (ATen binary_cross_entropy_with_logits)
+      const float l = (1.f - t) * x + (fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x))));
+      local += (double)l;
+      const float sg = 1.f / (1.f + expf(-x));
+      if (dpred) dpred[half * count + i] = gs * (sg - t);
+    } else if constexpr (OBJ == SN_GAN_MSE) {
+      const float d = x - t;
+      local += (double)(d * d);
+      if (dpred) dpred[half * count + i] = gs * (2.f * d);
+    } else {
+      local += (double)x;
+      if (dpred) dpred[half * count + i] = gs * t;
+    }
   }
   (void)halves;
+  if constexpr (OBJ == SN_GAN_WGAN) local *= (double)t;
   block_add_double(local / (double)count, loss_acc + half);
 }
 
@@ -2105,8 +2122,8 @@ int sn_bce_logits_fwd_bwd(const float* pred, long long count_per_half, int halve
                           float gscale, double* loss_acc, float* dpred, void* stream) {
   SN_REQUIRE(halves == 1 || halves == 2, "halves must be 1 or 2");
   dim3 grid(grid_for(count_per_half), halves);
-  bce_logits_kernel<<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, t0, t1, nullptr,
-                                                                   gscale, loss_acc, dpred);
+  gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, t0, t1,
+                                                                             nullptr, gscale, loss_acc, dpred);
   LAUNCH_CHECK();
   return SN_OK;
 }
@@ -2115,8 +2132,35 @@ int sn_bce_logits_fwd_bwd_dev(const float* pred, long long count_per_half, int h
                               float gscale, double* loss_acc, float* dpred, void* stream) {
   SN_REQUIRE((halves == 1 || halves == 2) && t_dev, "halves must be 1 or 2, t_dev non-null");
   dim3 grid(grid_for(count_per_half), halves);
-  bce_logits_kernel<<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, 0.f, 0.f, t_dev,
-                                                                   gscale, loss_acc, dpred);
+  gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, 0.f, 0.f,
+                                                                             t_dev, gscale, loss_acc, dpred);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_gan_loss_fwd_bwd_dev(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
+                            const float* t_dev, float gscale, double* loss_acc, float* dpred, void* stream) {
+  SN_REQUIRE(halves == 1 || halves == 2, "halves must be 1 or 2");
+  SN_REQUIRE(pred && loss_acc && count_per_half > 0, "gan_loss: null pointer or empty prediction");
+  SN_REQUIRE(objective != SN_GAN_WGAN || !t_dev, "gan_loss: the WGAN signs are passed by value (t0, t1), not t_dev");
+  dim3 grid(grid_for(count_per_half), halves);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (objective) {
+    case SN_GAN_BCE:
+      gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
+                                                              loss_acc, dpred);
+      break;
+    case SN_GAN_MSE:
+      gan_loss_kernel<SN_GAN_MSE><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
+                                                              loss_acc, dpred);
+      break;
+    case SN_GAN_WGAN:
+      gan_loss_kernel<SN_GAN_WGAN><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, nullptr, gscale,
+                                                               loss_acc, dpred);
+      break;
+    default:
+      SN_REQUIRE(false, "gan_loss: unknown objective %d", objective);
+  }
   LAUNCH_CHECK();
   return SN_OK;
 }

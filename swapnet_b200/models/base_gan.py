@@ -3,9 +3,12 @@
 Keeps the option surface and step order of /root/reference/models/base_gan.py:16-231:
     forward -> zero/backward/step D -> zero/backward/step G        (base_gan.py:194-203)
 with G = a generator engine, D = the conditional PatchGAN (define_D 'basic' / 'n_layers',
-discriminators.py:45-88), GANLoss = vanilla BCE-with-logits with the reference's smooth labels
-(loss.py:65-122, including the "fake target drawn from the real range" quirk, loss.py:102) and
-torch.optim.AdamW exactly as optimizers/__init__.py:37-60 builds it.
+discriminators.py:45-88), GANLoss (loss.py:12-130) for --gan_mode vanilla (BCE-with-logits), lsgan (MSE) and wgan
+(-mean(pred) for real, +mean(pred) for fake) and torch.optim.AdamW exactly as optimizers/__init__.py:37-60 builds it.
+vanilla and lsgan use the reference's smooth labels (loss.py:65-108, including the "fake target drawn from the real
+range" quirk, loss.py:102): three CPU-RNG draws per step, D_fake, D_real, G_gan.  wgan has no target and draws nothing.
+The wgan weight "clamp" of texture_model.py:132-135 (`p.data.clamp(...)`, not in place) leaves D unchanged in the
+reference and is not reproduced; the warp stage has none.
 
 What runs differently from the eager reference (results unchanged):
   * D's fake and real passes of the D step run as ONE batch of 2B with per-half targets (InstanceNorm is per
@@ -13,9 +16,10 @@ What runs differently from the eager reference (results unchanged):
   * D's weight gradients are not computed in the G step (the reference computes and discards
     them, SURVEY App. B #5);
   * losses stay on the device until get_current_losses() is called.
-Unsupported option values raise (there is no eager fallback): --gan_mode other than vanilla,
---gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch under data
-parallelism (no cross-rank batch statistics), --optimizer AdaBound.
+Unsupported option values raise (there is no eager fallback): --gan_mode wgan-gp / dragan-gp / dragan-lp (the
+gradient penalty needs a second derivative through D), --gan_mode mescheder-r1-gp / mescheder-r2-gp (the reference's
+GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch
+under data parallelism (no cross-rank batch statistics), --optimizer AdaBound.
 """
 from __future__ import annotations
 
@@ -112,8 +116,13 @@ class BaseGAN(BaseModel, ABC):
         # dedicated, identically seeded generator so that every rank sees the same label (SURVEY §8e i)
         self._labels = parallel.LabelDraws(1234 if self._world > 1 else None)
         if self.is_train:
-            if opt.gan_mode != "vanilla":
-                raise NotImplementedError(f"--gan_mode {opt.gan_mode}: only vanilla runs on the B200 engines")
+            if opt.gan_mode in ("wgan-gp", "dragan-gp", "dragan-lp"):
+                raise NotImplementedError(f"--gan_mode {opt.gan_mode}: its gradient penalty needs a second derivative "
+                                          "through D, which the engines do not compute (DESIGN.md §1)")
+            if opt.gan_mode not in ops.GAN_OBJECTIVES:
+                raise NotImplementedError(f"--gan_mode {opt.gan_mode}: the reference's GANLoss does not implement it "
+                                          "either (loss.py:61-62)")
+            self._gan_obj = ops.GAN_OBJECTIVES[opt.gan_mode]
             if opt.gan_label_mode != "smooth":
                 raise NotImplementedError("--gan_label_mode hard crashes in the reference (loss.py:92,101) and is "
                                           "not provided")
@@ -246,9 +255,19 @@ class BaseGAN(BaseModel, ABC):
         fp32 `rand(1) * (1.1 - 0.7) + 0.7`, for real AND fake targets."""
         return self._labels.draw()
 
-    def _targets(self, lo: int, hi: int) -> torch.Tensor:
-        """Device view of the smooth-label targets lo..hi-1 of the step-parameter buffer; drawn here (reference order)
-        when the phases are run by hand, by the step prologue inside optimize_parameters()."""
+    def label_draws(self) -> int:
+        """Smooth labels one training step draws: D_fake, D_real, G_gan for vanilla / lsgan; none for wgan, whose loss
+        has no target (loss.py:123-127), so the CPU generator is left where the reference leaves it."""
+        if not hasattr(self, "net_discriminator") or self._gan_obj == ops.GAN_WGAN:
+            return 0
+        return 3
+
+    def _targets(self, lo: int, hi: int, wgan_signs) -> object:
+        """Per-half scalars of the GAN loss calls lo..hi-1: with wgan the signs (+1 fake, -1 real), constants of the call
+        site; otherwise the device view of the smooth-label targets lo..hi-1 of the step-parameter buffer, drawn here
+        (reference order) when the phases are run by hand, by the step prologue inside optimize_parameters()."""
+        if self._gan_obj == ops.GAN_WGAN:
+            return wgan_signs
         if not self._sp_ready:
             ops.set_step_params(self._sp[lo:hi], [self.draw_label() for _ in range(lo, hi)])
         return self._sp[lo:hi]
@@ -275,20 +294,20 @@ class BaseGAN(BaseModel, ABC):
         d.pack()
         self.pack_D_inputs(d.din.batch_slice(0, B), d.din.batch_slice(B, B))
         pred = d.forward()
-        t = self._targets(0, 2)                                  # order: D_fake, D_real (loss.py:117,121)
-        ops.bce_logits_fwd_bwd(pred, 2, t, 0.0, 0.5, self._acc[0:2], self._dpred_d)
+        t = self._targets(0, 2, (1.0, -1.0))                     # order: D_fake, D_real (loss.py:117,121)
+        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 2, t, 0.5, self._acc[0:2], self._dpred_d)
         d.backward(self._dpred_d)
         self.allreduce_grads(d)
 
     def gan_backward_through_D(self) -> torch.Tensor:
-        """G phase: D(fake) with the updated D, BCE against a 'real' label, gradient back to the
+        """G phase: D(fake) with the updated D, the GAN objective against a 'real' target, gradient back to the
         discriminator input.  Returns d(loss_G_gan)/d(din) [B,S,S,pad64(cin)] (fp32 NHWC)."""
         g = self._eng_Dg
         g.training = self.training
         g.pack()
         pred = g.forward()
-        t = self._targets(2, 3)
-        ops.bce_logits_fwd_bwd(pred, 1, t, 0.0, float(self.opt.lambda_gan), self._acc[2:3], self._dpred_g)
+        t = self._targets(2, 3, (-1.0,))
+        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 1, t, float(self.opt.lambda_gan), self._acc[2:3], self._dpred_g)
         g.backward(self._dpred_g, wgrad=False)
         return g.dx_in
 
@@ -302,10 +321,10 @@ class BaseGAN(BaseModel, ABC):
             setattr(self, k, v)
 
     def _step_prologue(self, optimizers) -> None:
-        """Everything of a step that is decided on the host, written to the device with ONE tiny launch: the three
-        smooth labels (CPU RNG, reference order), the AdamW scalars of this step, the dropout step seed."""
+        """Everything of a step that is decided on the host, written to the device with ONE tiny launch: the smooth
+        labels (CPU RNG, reference order; none with wgan), the AdamW scalars of this step, the dropout step seed."""
         vals = [0.0] * 22
-        for i in range(3 if hasattr(self, "net_discriminator") else 0):
+        for i in range(self.label_draws()):
             vals[i] = self.draw_label()
         for off, name in ((4, "D"), (12, "G")):
             if name in optimizers:

@@ -772,6 +772,30 @@ def bce_logits_fwd_bwd(pred: torch.Tensor, halves: int, t0, t1: float, gscale: f
                                             _ptr(dpred), _stream()))
 
 
+# GANLoss objectives (include/swapnet_b200.h SN_GAN_*) and the --gan_mode values that select them
+GAN_BCE, GAN_MSE, GAN_WGAN = 0, 1, 2
+GAN_OBJECTIVES = {"vanilla": GAN_BCE, "lsgan": GAN_MSE, "wgan": GAN_WGAN}
+
+
+def gan_loss_fwd_bwd(objective: int, pred: torch.Tensor, halves: int, t, gscale: float, loss_acc: torch.Tensor,
+                     dpred: Optional[torch.Tensor]) -> None:
+    """GANLoss over `halves` (1 or 2) equal consecutive blocks of `pred`, one pass: loss_acc[h] += the unweighted batch
+    mean of block h, dpred <- gscale * d(mean)/d(pred).  t holds one scalar per block: the target label of GAN_BCE /
+    GAN_MSE, as a device float32 tensor (step-parameter buffer) or a sequence of floats; the sign of GAN_WGAN (+1 for a
+    fake block, -1 for a real one) as a sequence of floats."""
+    count = pred.numel() // halves
+    if torch.is_tensor(t):
+        assert objective != GAN_WGAN, "the WGAN signs are constants of the call, passed by value"
+        assert t.dtype == torch.float32 and t.numel() >= halves and t.is_cuda
+        t0 = t1 = 0.0
+        tptr = t.data_ptr()
+    else:
+        assert len(t) == halves
+        t0, t1, tptr = float(t[0]), float(t[-1]), None
+    check(_lib.load().sn_gan_loss_fwd_bwd_dev(objective, pred.data_ptr(), count, halves, t0, t1, tptr, gscale,
+                                              loss_acc.data_ptr(), _ptr(dpred), _stream()))
+
+
 def l1_loss_fwd_bwd(a: torch.Tensor, c: int, b_nchw: torch.Tensor, weight: float, loss_acc: torch.Tensor,
                     grad: torch.Tensor) -> None:
     n, h, w, pitch = a.shape
