@@ -133,6 +133,10 @@ typedef struct sn_wgrad_desc {
   int ngroups; int group_start[SN_MAX_TAPS]; int group_size[SN_MAX_TAPS];
   int ksplit;                            /* 0 = auto */
   int nsplit;
+  int deterministic;                     /* 1: the ksplit partials go to a workspace owned by the plan and are added into
+                                            out in split order by a second kernel (bit-identical on every run); the auto
+                                            ksplit is then computed for SN_NUM_SMS SMs whatever the device, so the
+                                            summation order depends on the shapes alone.  Needs distinct tap_off. */
 } sn_wgrad_desc;
 
 typedef struct sn_plan sn_plan; /* opaque; owns the encoded TMA descriptors of one launch */
@@ -146,6 +150,10 @@ int sn_plan_has_stats(const sn_plan* plan);
 /* launch geometry of a plan, for per-plan timing tables: out[0] = kind (0 tap GEMM, 1 weight gradient), then
  * tap GEMM: M tiles, N tiles, phases, block_n, A row chunk; weight gradient: grid x, y, z, block_n, Y row chunk */
 int sn_plan_geometry(const sn_plan* plan, int* out);
+/* device workspace bytes a plan owns (the split-K partials of a deterministic weight-gradient plan; 0 otherwise) */
+long long sn_plan_workspace_bytes(const sn_plan* plan);
+/* the split-K count sn_wgrad_plan_create would choose for desc on a device with sm_count SMs (host only) */
+int sn_wgrad_ksplit(const sn_wgrad_desc* desc, int sm_count);
 
 /* ------------------------------------------------------------------------------------------
  * operand packing
@@ -217,6 +225,17 @@ int sn_stats_finalize(double* stats, int count, int hw, float eps, void* stream)
 /* per-(n,c) (sum, sum of squares) over the plane, accumulated in fp64, without sn_stats_finalize's conversion */
 int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream);
 
+/* Deterministic variants (the *_det entry points, sn_norm_act_bwd_desc.det_slots): where the plain entry point adds
+ * per-block partial sums with floating-point atomics, these store each block's partial to its own slot of the
+ * caller's workspace `slots` (slots_cap doubles) and a second kernel adds the slots in index order, so the result is
+ * bit-identical on every run.  Two launches that may overlap must not share a workspace.  sn_det_slots(n, c): doubles
+ * of workspace enough for any of them whose output is [n][c] per-channel values (or a loss of n*c <= 2 terms). */
+long long sn_det_slots(int n, int c);
+int sn_plane_sums_det(const float* y, int pitch, int n, int hw, int c, double* stats, double* slots,
+                      long long slots_cap, void* stream);
+int sn_plane_stats_det(const float* y, int pitch, int n, int hw, int c, float eps, double* stats, double* slots,
+                       long long slots_cap, void* stream);
+
 /* BatchNorm2d(affine, track_running_stats) statistics (pix2pix / PatchGAN `--norm batch`).  The n samples form `groups`
  * consecutive groups of n/groups samples, each normalised as a call of its own (the discriminator's fake and real
  * halves).  Reductions over the samples run in sample order on one thread per channel: no atomics.
@@ -284,12 +303,16 @@ typedef struct sn_norm_act_bwd_desc {
   int bn_groups;                         /* sample groups of the forward call (sn_bn_finalize) */
   int bn_train;                          /* 1: batch statistics (dL/dy subtracts the group means); 0: running statistics */
   float* gamma_grad; float* beta_grad;   /* optional [c]: += d(loss)/d(gamma), d(loss)/d(beta) */
+  double* det_slots; long long det_slots_cap; /* non-NULL: deterministic gstats reduction (see sn_det_slots; no
+                                            fused bias_grad) */
 } sn_norm_act_bwd_desc;
 int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream);
 
 /* bias gradient db[c] = sum over the npix pixels of dL/dy (split planes); scratch: double[c] */
 int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
                  double* scratch, float* db, void* stream);
+int sn_bias_grad_det(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
+                     double* scratch, float* db, double* slots, long long slots_cap, void* stream);
 
 /* dst[n,h,w,c] = sum_i src_i (fp32), e.g. the residual-stream gradient of a ResidualBlock */
 int sn_sum_grads(const sn_grad_src* src, int nsrc, int n, int h, int w, int c, float* dst,
@@ -340,6 +363,9 @@ int sn_ce_loss_fwd_bwd(const float* logits, int pitch, const void* target, int t
 int sn_ce_tanh_bwd(const float* logits, int pitch, const void* target, int target_layout, const sn_grad_src* src,
                    int nsrc, int n, int h, int w, int c, float weight, double* loss_acc, void* dy_hi, void* dy_lo,
                    int dy_pitch, int dy_coff, int dy_fmt, void* stream);
+int sn_ce_tanh_bwd_det(const float* logits, int pitch, const void* target, int target_layout, const sn_grad_src* src,
+                       int nsrc, int n, int h, int w, int c, float weight, double* loss_acc, void* dy_hi, void* dy_lo,
+                       int dy_pitch, int dy_coff, int dy_fmt, double* slots, long long slots_cap, void* stream);
 /* BCEWithLogitsLoss(pred, t) over two consecutive halves of `count` elements each with its own
  * target (loss.py:58,110-122): loss_acc[half] += mean, dpred = gscale * (sigmoid(x) - t)/count. */
 int sn_bce_logits_fwd_bwd(const float* pred, long long count_per_half, int halves, float t0, float t1,
@@ -357,9 +383,15 @@ enum { SN_GAN_BCE = 0, SN_GAN_MSE = 1, SN_GAN_WGAN = 2 };
  * SN_GAN_BCE runs the kernel of sn_bce_logits_fwd_bwd(_dev). */
 int sn_gan_loss_fwd_bwd_dev(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
                             const float* t_dev, float gscale, double* loss_acc, float* dpred, void* stream);
+int sn_gan_loss_fwd_bwd_det(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
+                            const float* t_dev, float gscale, double* loss_acc, float* dpred, double* slots,
+                            long long slots_cap, void* stream);
 /* L1Loss(a, b) * weight (texture_model.py:168-170); a NHWC (pitch), b NCHW; grad wrt a. */
 int sn_l1_loss_fwd_bwd(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c,
                        float weight, double* loss_acc, float* grad, int grad_pitch, void* stream);
+int sn_l1_loss_fwd_bwd_det(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c, float weight,
+                           double* loss_acc, float* grad, int grad_pitch, double* slots, long long slots_cap,
+                           void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * one-output-channel conv (PatchGAN logits, discriminators.py:131) over a per-tap
@@ -379,6 +411,12 @@ int sn_to_one_fwd(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, lo
 int sn_to_one_wgrad(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
                     const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
                     void* stream);
+/* deterministic sn_to_one_wgrad: per-block partials of dw in `slots` (float, slots_cap of them;
+ * sn_to_one_wgrad_det_slots(c) are enough), added into dw in block order */
+int sn_to_one_wgrad_det(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
+                        const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
+                        float* slots, long long slots_cap, void* stream);
+long long sn_to_one_wgrad_det_slots(int c);
 int sn_to_one_dgrad(const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int n, int h, int w, int c,
                     const float* weight, int k, int pad, float* dx, int dx_pitch, void* stream);
 
@@ -403,10 +441,19 @@ int sn_relu_pool_bwd(const float* y, int y_pitch, const float* g_pool, int gp_pi
  * (gradient w.r.t. the post-ReLU feature; gscale carries the 2 of x <- 2x - 1). c in {64..512}, c % 4 == 0. */
 int sn_feat_loss_fwd_bwd(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c, double weight,
                          double gscale, double* loss_acc, float* dx, int pdx, void* stream);
+/* deterministic variant (see sn_det_slots: sn_det_slots(1, 1) slots are enough) */
+int sn_feat_loss_fwd_bwd_det(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c,
+                             double weight, double gscale, double* loss_acc, float* dx, int pdx, double* slots,
+                             long long slots_cap, void* stream);
 /* gram_matrix (perceptual.py:6-10) of the rows r = (b, ch): X_r[p] = src[b*s_n + ch*s_c + p*s_p];
  * gram: double [n*c][n*c] (zeroed here).  n*c <= 96. */
 int sn_gram(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix, double* gram,
             void* stream);
+/* deterministic variant: per-block partial Gram matrices in `slots` (sn_gram_det_slots(n*c) doubles are enough), added
+ * in block order.  sn_gram_mse is one block and needs no variant. */
+int sn_gram_det(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
+                double* gram, double* slots, long long slots_cap, void* stream);
+long long sn_gram_det_slots(int rows);
 /* *loss_acc += weight * MSELoss(gram_out, gram_tgt);  m[r][j] = d(that)/d(gram_out) + transpose (fp32). */
 int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double weight, double* loss_acc, float* m,
                 void* stream);

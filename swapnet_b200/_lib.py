@@ -59,7 +59,7 @@ class SnWgradDesc(C.Structure):
         ("rows_valid", C.c_int), ("cols_valid", C.c_int),
         ("block_n", C.c_int), ("y_chunk", C.c_int),
         ("ngroups", C.c_int), ("group_start", C.c_int * SN_MAX_TAPS), ("group_size", C.c_int * SN_MAX_TAPS),
-        ("ksplit", C.c_int), ("nsplit", C.c_int),
+        ("ksplit", C.c_int), ("nsplit", C.c_int), ("deterministic", C.c_int),
     ]
 
 
@@ -110,6 +110,7 @@ class SnNormActBwdDesc(C.Structure):
         ("dy_fmt", C.c_int), ("bias_grad", C.c_void_p),
         ("gamma", C.c_void_p), ("beta", C.c_void_p), ("bn_groups", C.c_int), ("bn_train", C.c_int),
         ("gamma_grad", C.c_void_p), ("beta_grad", C.c_void_p),
+        ("det_slots", C.c_void_p), ("det_slots_cap", C.c_longlong),
     ]
 
 
@@ -126,6 +127,18 @@ SIGNATURES = {
     "sn_plan_destroy": (None, [_VP]),
     "sn_plan_has_stats": (_I, [_VP]),
     "sn_plan_geometry": (_I, [_VP, C.POINTER(C.c_int)]),
+    "sn_plan_workspace_bytes": (_LL, [_VP]),
+    "sn_wgrad_ksplit": (_I, [C.POINTER(SnWgradDesc), _I]),
+    "sn_det_slots": (_LL, [_I, _I]),
+    "sn_plane_sums_det": (_I, [_VP, _I, _I, _I, _I, _VP, _VP, _LL, _VP]),
+    "sn_plane_stats_det": (_I, [_VP, _I, _I, _I, _I, _F, _VP, _VP, _LL, _VP]),
+    "sn_bias_grad_det": (_I, [_VP, _VP, _I, _I, _I, _LL, _I, _VP, _VP, _VP, _LL, _VP]),
+    "sn_ce_tanh_bwd_det": (_I, [_VP, _I, _VP, _I, C.POINTER(SnGradSrc), _I, _I, _I, _I, _I, _F, _VP, _VP, _VP, _I, _I,
+                                _I, _VP, _LL, _VP]),
+    "sn_gan_loss_fwd_bwd_det": (_I, [_I, _VP, _LL, _I, _F, _F, _VP, _F, _VP, _VP, _VP, _LL, _VP]),
+    "sn_l1_loss_fwd_bwd_det": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _F, _VP, _VP, _I, _VP, _LL, _VP]),
+    "sn_to_one_wgrad_det": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP, _VP, _LL, _VP]),
+    "sn_to_one_wgrad_det_slots": (_LL, [_I]),
     "sn_stats_finalize": (_I, [_VP, _I, _I, _F, _VP]),
     "sn_plane_sums": (_I, [_VP, _I, _I, _I, _I, _VP, _VP]),
     "sn_bn_finalize": (_I, [_VP, _I, _I, _I, _I, _F, _F, _VP, _VP, _VP, _VP]),
@@ -169,6 +182,9 @@ SIGNATURES = {
     "sn_relu_pool_bwd": (_I, [_VP, _I, _VP, _I, _VP, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_feat_loss_fwd_bwd": (_I, [_VP, _I, _VP, _I, _LL, _I, C.c_double, C.c_double, _VP, _VP, _I, _VP]),
     "sn_gram": (_I, [_VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP]),
+    "sn_gram_det": (_I, [_VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP, _LL, _VP]),
+    "sn_gram_det_slots": (_LL, [_I]),
+    "sn_feat_loss_fwd_bwd_det": (_I, [_VP, _I, _VP, _I, _LL, _I, C.c_double, C.c_double, _VP, _VP, _I, _VP, _LL, _VP]),
     "sn_gram_mse": (_I, [_VP, _VP, _I, C.c_double, _VP, _VP, _VP]),
     "sn_gram_bwd": (_I, [_VP, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _I, _I, _VP]),
     "sn_roi_align_pack_fwd": (_I, [_VP, _I, _I, _I, _I, _VP, _I, _I, _VP, _I, _VP, _VP, _I, _I, _I, _VP]),

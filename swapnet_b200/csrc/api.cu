@@ -86,8 +86,15 @@ int sn_plan_geometry(const sn_plan* plan, int* out) {
   return SN_OK;
 }
 
+long long sn_plan_workspace_bytes(const sn_plan* plan) {
+  return plan && plan->kind == 1 ? (long long)plan->wg.ws_bytes : 0;
+}
+
+int sn_wgrad_ksplit(const sn_wgrad_desc* desc, int sm_count) { return sn_wgrad_plan_ksplit(desc, sm_count); }
+
 void sn_plan_destroy(sn_plan* plan) {
   if (plan && plan->kind == 0 && plan->tg.p.tile_counter) cudaFree(plan->tg.p.tile_counter);
+  if (plan && plan->kind == 1 && plan->wg.p.det_ws) cudaFree(plan->wg.p.det_ws);
   delete plan;
 }
 

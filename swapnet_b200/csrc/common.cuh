@@ -325,4 +325,26 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// ---- deterministic reductions (the *_det entry points, sn_wgrad_desc.deterministic) -------------------------------
+// A reduction whose blocks would add their partials into dst[i] with floating-point atomics instead stores block s's
+// partial of output i to slots[s * count + i] with a plain store; det_sum_slots, launched next on the same stream, adds
+// the nslots partials of every output in slot order.  No block waits for another, and since the slot counts come from
+// the shapes alone, the summation order — and so every bit of the result — is the same on every run.
+template <typename T>
+__global__ void det_sum_slots_kernel(const T* __restrict__ slots, int nslots, long long count, T* __restrict__ dst) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count;
+       i += (long long)gridDim.x * blockDim.x) {
+    T s = slots[i];
+    for (int k = 1; k < nslots; ++k) s += slots[(long long)k * count + i];
+    dst[i] += s;
+  }
+}
+template <typename T>
+inline cudaError_t det_sum_slots(const T* slots, int nslots, long long count, T* dst, cudaStream_t st) {
+  long long g = (count + 255) / 256;
+  if (g > SN_NUM_SMS * 8) g = SN_NUM_SMS * 8;
+  det_sum_slots_kernel<T><<<(int)(g < 1 ? 1 : g), 256, 0, st>>>(slots, nslots, count, dst);
+  return cudaGetLastError();
+}
+
 #endif  // __CUDACC__

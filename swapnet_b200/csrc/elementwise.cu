@@ -492,9 +492,10 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const sn_pack_i
 // ---------------------------------------------------------------------------------
 __device__ __forceinline__ double atomic_add_f64(double* a, double v) { return atomicAdd(a, v); }
 
-// grid (ceil(C/32), slabs, N), block (32, 8)
+// grid (ceil(C/32), slabs, N), block (32, 8).  DET: the slab's partials go to slot blockIdx.y (det_sum_slots)
+template <bool DET>
 __global__ void plane_stats_kernel(const float* __restrict__ y, int pitch, int hw, int C,
-                                   double* __restrict__ stats) {
+                                   double* __restrict__ stats, double* __restrict__ slots) {
   __shared__ float s1s[8][33], s2s[8][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   const int n = blockIdx.z;
@@ -520,8 +521,15 @@ __global__ void plane_stats_kernel(const float* __restrict__ y, int pitch, int h
       a += (double)s1s[j][threadIdx.x];
       b += (double)s2s[j][threadIdx.x];
     }
-    atomic_add_f64(&stats[((long long)n * C + c) * 2 + 0], a);
-    atomic_add_f64(&stats[((long long)n * C + c) * 2 + 1], b);
+    const long long i = ((long long)n * C + c) * 2;
+    if constexpr (DET) {
+      double* sl = slots + (long long)blockIdx.y * (2LL * gridDim.z * C);
+      sl[i] = a;
+      sl[i + 1] = b;
+    } else {
+      atomic_add_f64(&stats[i + 0], a);
+      atomic_add_f64(&stats[i + 1], b);
+    }
   }
 }
 // (sum, sumsq) -> (mean, rstd), biased variance (torch instance_norm)
@@ -618,8 +626,10 @@ __global__ void bn_bwd_group_kernel(double* g, int N, int C, int groups, int hw,
 
 
 // bias gradient: db[c] = sum over pixels of dy (dy carried as split planes)
+template <bool DET>
 __global__ void bias_grad_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo,
-                                 int pitch, int fmt, long long npix, int C, double* __restrict__ acc) {
+                                 int pitch, int fmt, long long npix, int C, double* __restrict__ acc,
+                                 double* __restrict__ slots) {
   __shared__ float s1s[8][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   const long long per = (npix + gridDim.y - 1) / gridDim.y;
@@ -643,12 +653,15 @@ __global__ void bias_grad_kernel(const uint16_t* __restrict__ hi, const uint16_t
     double a = 0.0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) a += (double)s1s[j][threadIdx.x];
-    atomic_add_f64(&acc[c], a);
+    if constexpr (DET) slots[(long long)blockIdx.y * C + c] = a;
+    else atomic_add_f64(&acc[c], a);
   }
 }
 // 8 channels per thread (one 16-B load per plane); block (G = C/8 groups, 256/G pixel rows)
+template <bool DET>
 __global__ void bias_grad_v8_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo, int pitch,
-                                    int fmt, long long npix, int C, double* __restrict__ acc) {
+                                    int fmt, long long npix, int C, double* __restrict__ acc,
+                                    double* __restrict__ slots) {
   __shared__ float red[256][8];
   const int gch = blockIdx.x * blockDim.x + threadIdx.x;   // channel group
   const int c = gch * 8;
@@ -687,7 +700,8 @@ __global__ void bias_grad_v8_kernel(const uint16_t* __restrict__ hi, const uint1
       if (c + j >= C) break;
       double u = 0.0;
       for (int r = 0; r < (int)blockDim.y; ++r) u += (double)red[r * blockDim.x + threadIdx.x][j];
-      atomic_add_f64(&acc[c + j], u);
+      if constexpr (DET) slots[(long long)blockIdx.y * C + c + j] = u;
+      else atomic_add_f64(&acc[c + j], u);
     }
   }
 }
@@ -844,6 +858,7 @@ struct NormActBwdArgs {
   uint16_t* hi; uint16_t* lo; int dy_pitch, dy_coff, fmt;
   float* bias_grad;   // optional [C]: += per-channel sums of the dy written (the conv's bias gradient)
   const float* gamma; const float* beta;   // BatchNorm affine (AFF instantiations): the gate is on gamma*xhat + beta
+  double* slots;      // DET reduce instantiations: per-slab partials of gstats (det_sum_slots)
 };
 
 // gradient w.r.t. xhat (before the InstanceNorm backward), and xhat itself
@@ -869,6 +884,7 @@ __device__ __forceinline__ float grad_xhat(const NormActBwdArgs& a, unsigned lon
 }
 
 // grid (ceil(C/32), slabs, N), block (32, 8): sums of g and g*xhat per (n, c)
+template <bool DET>
 __global__ void norm_act_bwd_reduce_kernel(const NormActBwdArgs a) {
   __shared__ float s1s[8][33], s2s[8][33];
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
@@ -898,8 +914,15 @@ __global__ void norm_act_bwd_reduce_kernel(const NormActBwdArgs a) {
       u += (double)s1s[j][threadIdx.x];
       v += (double)s2s[j][threadIdx.x];
     }
-    atomic_add_f64(&a.gstats[((long long)n * a.C + c) * 2 + 0], u);
-    atomic_add_f64(&a.gstats[((long long)n * a.C + c) * 2 + 1], v);
+    const long long i = ((long long)n * a.C + c) * 2;
+    if constexpr (DET) {
+      double* sl = a.slots + (long long)blockIdx.y * (2LL * gridDim.z * a.C);
+      sl[i] = u;
+      sl[i + 1] = v;
+    } else {
+      atomic_add_f64(&a.gstats[i + 0], u);
+      atomic_add_f64(&a.gstats[i + 1], v);
+    }
   }
 }
 
@@ -1048,7 +1071,9 @@ __global__ void dropout_mask_kernel(unsigned long long seed, uint32_t thresh, lo
 // ---------------------------------------------------------------------------------
 // losses
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ void block_add_double(double v, double* dst) {
+// DET: the block's sum goes to slots[blockIdx.x * gridDim.y + blockIdx.y] (det_sum_slots over gridDim.x slots)
+template <bool DET>
+__device__ __forceinline__ void block_add_double(double v, double* dst, double* slots) {
   __shared__ double red[32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -1059,7 +1084,10 @@ __device__ __forceinline__ void block_add_double(double v, double* dst) {
     v = lane < (blockDim.x >> 5) ? red[lane] : 0.0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) atomicAdd(dst, v);
+    if (lane == 0) {
+      if constexpr (DET) slots[(long long)blockIdx.x * gridDim.y + blockIdx.y] = v;
+      else atomicAdd(dst, v);
+    }
   }
 }
 
@@ -1101,19 +1129,20 @@ __global__ void ce_loss_kernel(const float* __restrict__ logits, int pitch,
       grad[pix * gpitch + c] = scale * (sm - (c == arg ? 1.f : 0.f));
     }
   }
-  block_add_double(local * (double)weight / (double)npix, loss_acc);
+  block_add_double<false>(local * (double)weight / (double)npix, loss_acc, nullptr);
 }
 
 // CE on the tanh head fused with the head's own backward (warp_model.py:147-150 + swapnet_modules.py:85-90): per pixel
 //   g_c  = weight/npix * (softmax(o)_c - [c == argmax target])  +  sum of the extra gradient sources (the GAN term),
 //   dy_c = g_c * (1 - o_c^2)          written as split planes (channels c..pad8 zero-filled, 16-byte stores)
 // replaces ce_loss + tanh_bwd: the 19-channel logits are read once and the fp32 CE gradient never touches HBM.
+template <bool DET>
 __global__ void __launch_bounds__(128) ce_tanh_bwd_kernel(const float* __restrict__ logits, int pitch,
                                                           const float* __restrict__ target,
                                                           const uint8_t* __restrict__ label, const GradSrcs g, int N,
                                                           int H, int W, int C, float weight, double* loss_acc,
                                                           uint16_t* __restrict__ hi, uint16_t* __restrict__ lo,
-                                                          int dy_pitch, int dy_coff, int fmt) {
+                                                          int dy_pitch, int dy_coff, int fmt, double* slots) {
   const long long npix = (long long)N * H * W;
   const long long HW = (long long)H * W;
   double local = 0.0;
@@ -1168,7 +1197,7 @@ __global__ void __launch_bounds__(128) ce_tanh_bwd_kernel(const float* __restric
       if (lo) *reinterpret_cast<uint4*>(lo + off) = b;
     }
   }
-  block_add_double(local * (double)weight / (double)npix, loss_acc);
+  block_add_double<DET>(local * (double)weight / (double)npix, loss_acc, slots);
 }
 
 // GANLoss (loss.py:110-130) over `halves` consecutive blocks of `count` predictions, one per blockIdx.y, each with its own
@@ -1177,10 +1206,10 @@ __global__ void __launch_bounds__(128) ce_tanh_bwd_kernel(const float* __restric
 //   SN_GAN_BCE   BCEWithLogitsLoss(x, t)      dL/dx = (sigmoid(x) - t) / count
 //   SN_GAN_MSE   MSELoss(x, t)                dL/dx = 2 (x - t) / count
 //   SN_GAN_WGAN  t * mean(x), t = +1 / -1     dL/dx = t / count            (t is a sign, not a label)
-template <int OBJ>
+template <int OBJ, bool DET>
 __global__ void gan_loss_kernel(const float* __restrict__ pred, long long count, int halves, float t0, float t1,
                                 const float* __restrict__ t_dev, float gscale, double* loss_acc,
-                                float* __restrict__ dpred) {
+                                float* __restrict__ dpred, double* slots) {
   const int half = blockIdx.y;
   const float t = t_dev ? t_dev[half] : (half == 0 ? t0 : t1);
   double local = 0.0;
@@ -1205,12 +1234,13 @@ __global__ void gan_loss_kernel(const float* __restrict__ pred, long long count,
   }
   (void)halves;
   if constexpr (OBJ == SN_GAN_WGAN) local *= (double)t;
-  block_add_double(local / (double)count, loss_acc + half);
+  block_add_double<DET>(local / (double)count, loss_acc + half, slots);
 }
 
+template <bool DET>
 __global__ void l1_loss_kernel(const float* __restrict__ a, int pitch, const float* __restrict__ b,
                                int N, int H, int W, int C, float weight, double* loss_acc,
-                               float* __restrict__ grad, int gpitch) {
+                               float* __restrict__ grad, int gpitch, double* slots) {
   const long long HW = (long long)H * W;
   const long long total = (long long)N * HW * C;
   double local = 0.0;
@@ -1224,7 +1254,7 @@ __global__ void l1_loss_kernel(const float* __restrict__ a, int pitch, const flo
     local += (double)fabsf(d);
     grad[pix * gpitch + c] = d > 0.f ? gs : (d < 0.f ? -gs : 0.f);
   }
-  block_add_double(local * (double)weight / (double)total, loss_acc);
+  block_add_double<DET>(local * (double)weight / (double)total, loss_acc, slots);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1462,7 +1492,7 @@ __device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned lon
 
 // grid (ceil(Q/bx), slabs, N), block (bx, 256/bx) with bx = min(32, pow2 >= Q): thread = channel quad,
 // strided over pixels (C = 64 layers — the largest tensors — use bx = 16, 16 pixel rows)
-template <bool AFF>
+template <bool AFF, bool DET>
 __global__ void __launch_bounds__(256, 4) norm_act_bwd_reduce_v4_kernel(const NormActBwdArgs a) {
   __shared__ float red[256][8];
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
@@ -1509,8 +1539,15 @@ __global__ void __launch_bounds__(256, 4) norm_act_bwd_reduce_v4_kernel(const No
         u += (double)red[r * blockDim.x + threadIdx.x][j];
         v += (double)red[r * blockDim.x + threadIdx.x][4 + j];
       }
-      atomic_add_f64(&a.gstats[((long long)n * a.C + c + j) * 2 + 0], u);
-      atomic_add_f64(&a.gstats[((long long)n * a.C + c + j) * 2 + 1], v);
+      const long long i = ((long long)n * a.C + c + j) * 2;
+      if constexpr (DET) {
+        double* sl = a.slots + (long long)blockIdx.y * (2LL * gridDim.z * a.C);
+        sl[i] = u;
+        sl[i + 1] = v;
+      } else {
+        atomic_add_f64(&a.gstats[i + 0], u);
+        atomic_add_f64(&a.gstats[i + 1], v);
+      }
     }
   }
 }
@@ -1781,17 +1818,49 @@ int sn_plane_stats(const float* y, int pitch, int n, int hw, int c, float eps, d
   return sn_stats_finalize(stats, n * c, hw, eps, stream);
 }
 
-int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream) {
+int sn_plane_stats_det(const float* y, int pitch, int n, int hw, int c, float eps, double* stats, double* slots,
+                       long long slots_cap, void* stream) {
+  const int rc = sn_plane_sums_det(y, pitch, n, hw, c, stats, slots, slots_cap, stream);
+  if (rc) return rc;
+  return sn_stats_finalize(stats, n * c, hw, eps, stream);
+}
+
+static int plane_sums_impl(const float* y, int pitch, int n, int hw, int c, double* stats, double* slots,
+                           long long slots_cap, cudaStream_t st) {
   SN_REQUIRE(y && stats, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
   SN_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 2 * n * c, st));
   const int cg = (c + 31) / 32;
   int slabs = (SN_NUM_SMS * 4 + n * cg - 1) / (n * cg);
   if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
   if (slabs < 1) slabs = 1;
-  plane_stats_kernel<<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats);
+  if (!slots) {
+    plane_stats_kernel<false><<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE((long long)slabs * 2 * n * c <= slots_cap, "plane_sums_det: %lld slots needed, %lld given",
+             (long long)slabs * 2 * n * c, slots_cap);
+  plane_stats_kernel<true><<<dim3(cg, slabs, n), dim3(32, 8), 0, st>>>(y, pitch, hw, c, stats, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, slabs, 2LL * n * c, stats, st));
   LAUNCH_CHECK();
   return SN_OK;
+}
+
+int sn_plane_sums(const float* y, int pitch, int n, int hw, int c, double* stats, void* stream) {
+  return plane_sums_impl(y, pitch, n, hw, c, stats, nullptr, 0, (cudaStream_t)stream);
+}
+
+int sn_plane_sums_det(const float* y, int pitch, int n, int hw, int c, double* stats, double* slots,
+                      long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "plane_sums_det: null slots");
+  return plane_sums_impl(y, pitch, n, hw, c, stats, slots, slots_cap, (cudaStream_t)stream);
+}
+
+long long sn_det_slots(int n, int c) {
+  // every *_det reduction but the weight gradients' runs slabs * g <= 6 * SN_NUM_SMS + g blocks per sample, where one
+  // block covers at most 256 channels of the output
+  return 2LL * 6 * SN_NUM_SMS * 256 + 2LL * n * c + 2LL * SN_NUM_SMS * 16;
 }
 
 int sn_bn_finalize(double* stats, int n, int c, int groups, int hw, float eps, float momentum, float* running_mean,
@@ -1897,7 +1966,10 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
   a.dy_pitch = d->dy_pitch; a.dy_coff = d->dy_coff; a.fmt = d->dy_fmt;
   a.bias_grad = d->bias_grad;
   a.gamma = d->gamma; a.beta = d->beta;
+  a.slots = d->det_slots;
   const bool aff = d->gamma != nullptr;
+  const bool det = d->det_slots != nullptr;
+  SN_REQUIRE(!det || !d->bias_grad, "norm_act_bwd: the deterministic reduction has no fused bias gradient");
   SN_REQUIRE((d->gamma == nullptr) == (d->beta == nullptr), "norm_act_bwd: gamma and beta go together");
   SN_REQUIRE(!aff || (d->stats && d->bn_groups >= 1 && d->n % d->bn_groups == 0 && !d->bias_grad),
              "norm_act_bwd: the BatchNorm variant needs stats, bn_groups dividing n, and no fused bias gradient");
@@ -1909,6 +1981,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
   if (d->stats) {
     SN_REQUIRE(d->gstats, "InstanceNorm backward needs gstats scratch");
     SN_CHECK_CUDA(cudaMemsetAsync(d->gstats, 0, sizeof(double) * 2 * d->n * d->c, st));
+    int nslabs = 1;
     if (vec) {
       int bx = 1;
       while (bx < d->c / 4 && bx < 32) bx <<= 1;
@@ -1916,16 +1989,28 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       int slabs = (SN_NUM_SMS * 6 + d->n * qg - 1) / (d->n * qg);
       if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
       if (slabs < 1) slabs = 1;
-      if (aff) norm_act_bwd_reduce_v4_kernel<true><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
-      else norm_act_bwd_reduce_v4_kernel<false><<<dim3(qg, slabs, d->n), dim3(bx, 256 / bx), 0, st>>>(a);
+      nslabs = slabs;
+      const dim3 grid(qg, slabs, d->n), blk(bx, 256 / bx);
+      if (det) SN_REQUIRE((long long)slabs * 2 * d->n * d->c <= d->det_slots_cap, "norm_act_bwd: det_slots too small");
+      if (aff && det) norm_act_bwd_reduce_v4_kernel<true, true><<<grid, blk, 0, st>>>(a);
+      else if (aff) norm_act_bwd_reduce_v4_kernel<true, false><<<grid, blk, 0, st>>>(a);
+      else if (det) norm_act_bwd_reduce_v4_kernel<false, true><<<grid, blk, 0, st>>>(a);
+      else norm_act_bwd_reduce_v4_kernel<false, false><<<grid, blk, 0, st>>>(a);
     } else {
       const int cg = (d->c + 31) / 32;
       int slabs = (SN_NUM_SMS * 4 + d->n * cg - 1) / (d->n * cg);
       if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
       if (slabs < 1) slabs = 1;
-      norm_act_bwd_reduce_kernel<<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
+      nslabs = slabs;
+      if (det) SN_REQUIRE((long long)slabs * 2 * d->n * d->c <= d->det_slots_cap, "norm_act_bwd: det_slots too small");
+      if (det) norm_act_bwd_reduce_kernel<true><<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
+      else norm_act_bwd_reduce_kernel<false><<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
     }
     LAUNCH_CHECK();
+    if (det) {
+      SN_CHECK_CUDA(det_sum_slots(d->det_slots, nslabs, 2LL * d->n * d->c, d->gstats, st));
+      LAUNCH_CHECK();
+    }
     if (aff)
       bn_bwd_group_kernel<<<(d->c + 127) / 128, 128, 0, st>>>(d->gstats, d->n, d->c, d->bn_groups, hw, d->bn_train,
                                                               d->gamma_grad, d->beta_grad);
@@ -1953,10 +2038,9 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
 }
 
 
-int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
-                 double* scratch, float* db, void* stream) {
+static int bias_grad_impl(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
+                          double* scratch, float* db, double* slots, long long slots_cap, cudaStream_t st) {
   SN_REQUIRE(dy_hi && scratch && db, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
   SN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * c, st));
   const int cg = (c + 31) / 32;
   long long slabs = (SN_NUM_SMS * 4 + cg - 1) / cg;
@@ -1974,13 +2058,40 @@ int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int 
     long long sl = (SN_NUM_SMS * 6 + gx - 1) / gx;
     if (sl > (npix + 255) / 256) sl = (npix + 255) / 256;
     if (sl < 1) sl = 1;
-    bias_grad_v8_kernel<<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch);
-  } else
-  bias_grad_kernel<<<dim3(cg, (int)slabs), dim3(32, 8), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch);
+    slabs = sl;
+    SN_REQUIRE(!slots || slabs * c <= slots_cap, "bias_grad_det: %lld slots needed, %lld given", slabs * c, slots_cap);
+    if (slots)
+      bias_grad_v8_kernel<true><<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch,
+                                                                                 slots);
+    else
+      bias_grad_v8_kernel<false><<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch,
+                                                                                  nullptr);
+  } else {
+    SN_REQUIRE(!slots || slabs * c <= slots_cap, "bias_grad_det: %lld slots needed, %lld given", slabs * c, slots_cap);
+    if (slots)
+      bias_grad_kernel<true><<<dim3(cg, (int)slabs), dim3(32, 8), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, slots);
+    else
+      bias_grad_kernel<false><<<dim3(cg, (int)slabs), dim3(32, 8), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, nullptr);
+  }
   LAUNCH_CHECK();
+  if (slots) {
+    SN_CHECK_CUDA(det_sum_slots(slots, (int)slabs, (long long)c, scratch, st));
+    LAUNCH_CHECK();
+  }
   bias_grad_finalize_kernel<<<(c + 255) / 256, 256, 0, st>>>(scratch, c, db);
   LAUNCH_CHECK();
   return SN_OK;
+}
+
+int sn_bias_grad(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
+                 double* scratch, float* db, void* stream) {
+  return bias_grad_impl(dy_hi, dy_lo, pitch, coff, fmt, npix, c, scratch, db, nullptr, 0, (cudaStream_t)stream);
+}
+
+int sn_bias_grad_det(const void* dy_hi, const void* dy_lo, int pitch, int coff, int fmt, long long npix, int c,
+                     double* scratch, float* db, double* slots, long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "bias_grad_det: null slots");
+  return bias_grad_impl(dy_hi, dy_lo, pitch, coff, fmt, npix, c, scratch, db, slots, slots_cap, (cudaStream_t)stream);
 }
 
 int sn_sum_grads(const sn_grad_src* src, int nsrc, int n, int h, int w, int c, float* dst,
@@ -2095,9 +2206,10 @@ int sn_ce_loss_fwd_bwd(const float* logits, int pitch, const void* target, int t
   return SN_OK;
 }
 
-int sn_ce_tanh_bwd(const float* logits, int pitch, const void* target, int target_layout, const sn_grad_src* src,
-                   int nsrc, int n, int h, int w, int c, float weight, double* loss_acc, void* dy_hi, void* dy_lo,
-                   int dy_pitch, int dy_coff, int dy_fmt, void* stream) {
+static int ce_tanh_bwd_impl(const float* logits, int pitch, const void* target, int target_layout,
+                            const sn_grad_src* src, int nsrc, int n, int h, int w, int c, float weight, double* loss_acc,
+                            void* dy_hi, void* dy_lo, int dy_pitch, int dy_coff, int dy_fmt, double* slots,
+                            long long slots_cap, cudaStream_t st) {
   SN_REQUIRE(c <= kMaxCE && logits && dy_hi && loss_acc, "ce_tanh_bwd: bad arguments (at most %d classes)", kMaxCE);
   SN_REQUIRE(target_layout == SN_LAYOUT_NCHW || target_layout == SN_LAYOUT_LABEL_U8,
              "ce_tanh_bwd: target must be NCHW fp32 or a uint8 label map");
@@ -2111,19 +2223,46 @@ int sn_ce_tanh_bwd(const float* logits, int pitch, const void* target, int targe
     if (rc) return rc;
   }
   const bool lab = target_layout == SN_LAYOUT_LABEL_U8;
-  ce_tanh_bwd_kernel<<<grid_for((long long)n * h * w, 128), 128, 0, (cudaStream_t)stream>>>(
-      logits, pitch, lab ? nullptr : (const float*)target, lab ? (const uint8_t*)target : nullptr, g, n, h, w, c, weight,
-      loss_acc, (uint16_t*)dy_hi, (uint16_t*)dy_lo, dy_pitch, dy_coff, dy_fmt);
+  const int blocks = grid_for((long long)n * h * w, 128);
+  const float* tf = lab ? nullptr : (const float*)target;
+  const uint8_t* tl = lab ? (const uint8_t*)target : nullptr;
+  if (!slots) {
+    ce_tanh_bwd_kernel<false><<<blocks, 128, 0, st>>>(logits, pitch, tf, tl, g, n, h, w, c, weight, loss_acc,
+                                                      (uint16_t*)dy_hi, (uint16_t*)dy_lo, dy_pitch, dy_coff, dy_fmt,
+                                                      nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE(blocks <= slots_cap, "ce_tanh_bwd_det: %d slots needed, %lld given", blocks, slots_cap);
+  ce_tanh_bwd_kernel<true><<<blocks, 128, 0, st>>>(logits, pitch, tf, tl, g, n, h, w, c, weight, loss_acc,
+                                                   (uint16_t*)dy_hi, (uint16_t*)dy_lo, dy_pitch, dy_coff, dy_fmt, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, blocks, 1, loss_acc, st));
   LAUNCH_CHECK();
   return SN_OK;
+}
+
+int sn_ce_tanh_bwd(const float* logits, int pitch, const void* target, int target_layout, const sn_grad_src* src,
+                   int nsrc, int n, int h, int w, int c, float weight, double* loss_acc, void* dy_hi, void* dy_lo,
+                   int dy_pitch, int dy_coff, int dy_fmt, void* stream) {
+  return ce_tanh_bwd_impl(logits, pitch, target, target_layout, src, nsrc, n, h, w, c, weight, loss_acc, dy_hi, dy_lo,
+                          dy_pitch, dy_coff, dy_fmt, nullptr, 0, (cudaStream_t)stream);
+}
+
+int sn_ce_tanh_bwd_det(const float* logits, int pitch, const void* target, int target_layout, const sn_grad_src* src,
+                       int nsrc, int n, int h, int w, int c, float weight, double* loss_acc, void* dy_hi, void* dy_lo,
+                       int dy_pitch, int dy_coff, int dy_fmt, double* slots, long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "ce_tanh_bwd_det: null slots");
+  return ce_tanh_bwd_impl(logits, pitch, target, target_layout, src, nsrc, n, h, w, c, weight, loss_acc, dy_hi, dy_lo,
+                          dy_pitch, dy_coff, dy_fmt, slots, slots_cap, (cudaStream_t)stream);
 }
 
 int sn_bce_logits_fwd_bwd(const float* pred, long long count_per_half, int halves, float t0, float t1,
                           float gscale, double* loss_acc, float* dpred, void* stream) {
   SN_REQUIRE(halves == 1 || halves == 2, "halves must be 1 or 2");
   dim3 grid(grid_for(count_per_half), halves);
-  gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, t0, t1,
-                                                                             nullptr, gscale, loss_acc, dpred);
+  gan_loss_kernel<SN_GAN_BCE, false><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, t0, t1,
+                                                                             nullptr, gscale, loss_acc, dpred, nullptr);
   LAUNCH_CHECK();
   return SN_OK;
 }
@@ -2132,45 +2271,103 @@ int sn_bce_logits_fwd_bwd_dev(const float* pred, long long count_per_half, int h
                               float gscale, double* loss_acc, float* dpred, void* stream) {
   SN_REQUIRE((halves == 1 || halves == 2) && t_dev, "halves must be 1 or 2, t_dev non-null");
   dim3 grid(grid_for(count_per_half), halves);
-  gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, 0.f, 0.f,
-                                                                             t_dev, gscale, loss_acc, dpred);
+  gan_loss_kernel<SN_GAN_BCE, false><<<grid, kEwThreads, 0, (cudaStream_t)stream>>>(pred, count_per_half, halves, 0.f, 0.f,
+                                                                             t_dev, gscale, loss_acc, dpred, nullptr);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+}  // extern "C"
+
+template <bool DET>
+static void launch_gan_loss(int objective, dim3 grid, cudaStream_t s, const float* pred, long long count_per_half,
+                            int halves, float t0, float t1, const float* t_dev, float gscale, double* loss_acc,
+                            float* dpred, double* slots) {
+  switch (objective) {
+    case SN_GAN_BCE:
+      gan_loss_kernel<SN_GAN_BCE, DET><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
+                                                                   loss_acc, dpred, slots);
+      break;
+    case SN_GAN_MSE:
+      gan_loss_kernel<SN_GAN_MSE, DET><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
+                                                                   loss_acc, dpred, slots);
+      break;
+    default:
+      gan_loss_kernel<SN_GAN_WGAN, DET><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, nullptr,
+                                                                    gscale, loss_acc, dpred, slots);
+  }
+}
+
+extern "C" {
+
+static int gan_loss_impl(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
+                         const float* t_dev, float gscale, double* loss_acc, float* dpred, double* slots,
+                         long long slots_cap, cudaStream_t s) {
+  SN_REQUIRE(halves == 1 || halves == 2, "halves must be 1 or 2");
+  SN_REQUIRE(pred && loss_acc && count_per_half > 0, "gan_loss: null pointer or empty prediction");
+  SN_REQUIRE(objective != SN_GAN_WGAN || !t_dev, "gan_loss: the WGAN signs are passed by value (t0, t1), not t_dev");
+  SN_REQUIRE(objective == SN_GAN_BCE || objective == SN_GAN_MSE || objective == SN_GAN_WGAN,
+             "gan_loss: unknown objective %d", objective);
+  dim3 grid(grid_for(count_per_half), halves);
+  if (!slots) {
+    launch_gan_loss<false>(objective, grid, s, pred, count_per_half, halves, t0, t1, t_dev, gscale, loss_acc, dpred,
+                           nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE((long long)grid.x * halves <= slots_cap, "gan_loss_det: slots too small");
+  launch_gan_loss<true>(objective, grid, s, pred, count_per_half, halves, t0, t1, t_dev, gscale, loss_acc, dpred, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, (int)grid.x, (long long)halves, loss_acc, s));
   LAUNCH_CHECK();
   return SN_OK;
 }
 
 int sn_gan_loss_fwd_bwd_dev(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
                             const float* t_dev, float gscale, double* loss_acc, float* dpred, void* stream) {
-  SN_REQUIRE(halves == 1 || halves == 2, "halves must be 1 or 2");
-  SN_REQUIRE(pred && loss_acc && count_per_half > 0, "gan_loss: null pointer or empty prediction");
-  SN_REQUIRE(objective != SN_GAN_WGAN || !t_dev, "gan_loss: the WGAN signs are passed by value (t0, t1), not t_dev");
-  dim3 grid(grid_for(count_per_half), halves);
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (objective) {
-    case SN_GAN_BCE:
-      gan_loss_kernel<SN_GAN_BCE><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
-                                                              loss_acc, dpred);
-      break;
-    case SN_GAN_MSE:
-      gan_loss_kernel<SN_GAN_MSE><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, t_dev, gscale,
-                                                              loss_acc, dpred);
-      break;
-    case SN_GAN_WGAN:
-      gan_loss_kernel<SN_GAN_WGAN><<<grid, kEwThreads, 0, s>>>(pred, count_per_half, halves, t0, t1, nullptr, gscale,
-                                                               loss_acc, dpred);
-      break;
-    default:
-      SN_REQUIRE(false, "gan_loss: unknown objective %d", objective);
+  return gan_loss_impl(objective, pred, count_per_half, halves, t0, t1, t_dev, gscale, loss_acc, dpred, nullptr, 0,
+                       (cudaStream_t)stream);
+}
+
+int sn_gan_loss_fwd_bwd_det(int objective, const float* pred, long long count_per_half, int halves, float t0, float t1,
+                            const float* t_dev, float gscale, double* loss_acc, float* dpred, double* slots,
+                            long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "gan_loss_det: null slots");
+  return gan_loss_impl(objective, pred, count_per_half, halves, t0, t1, t_dev, gscale, loss_acc, dpred, slots, slots_cap,
+                       (cudaStream_t)stream);
+}
+
+static int l1_loss_impl(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c, float weight,
+                        double* loss_acc, float* grad, int grad_pitch, double* slots, long long slots_cap,
+                        cudaStream_t st) {
+  const int blocks = grid_for((long long)n * h * w * c);
+  if (!slots) {
+    l1_loss_kernel<false><<<blocks, kEwThreads, 0, st>>>(a, pitch, b_nchw, n, h, w, c, weight, loss_acc, grad,
+                                                         grad_pitch, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
   }
+  SN_REQUIRE(blocks <= slots_cap, "l1_loss_det: %d slots needed, %lld given", blocks, slots_cap);
+  l1_loss_kernel<true><<<blocks, kEwThreads, 0, st>>>(a, pitch, b_nchw, n, h, w, c, weight, loss_acc, grad, grad_pitch,
+                                                      slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, blocks, 1, loss_acc, st));
   LAUNCH_CHECK();
   return SN_OK;
 }
 
 int sn_l1_loss_fwd_bwd(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c,
                        float weight, double* loss_acc, float* grad, int grad_pitch, void* stream) {
-  l1_loss_kernel<<<grid_for((long long)n * h * w * c), kEwThreads, 0, (cudaStream_t)stream>>>(
-      a, pitch, b_nchw, n, h, w, c, weight, loss_acc, grad, grad_pitch);
-  LAUNCH_CHECK();
-  return SN_OK;
+  return l1_loss_impl(a, pitch, b_nchw, n, h, w, c, weight, loss_acc, grad, grad_pitch, nullptr, 0,
+                      (cudaStream_t)stream);
+}
+
+int sn_l1_loss_fwd_bwd_det(const float* a, int pitch, const float* b_nchw, int n, int h, int w, int c, float weight,
+                           double* loss_acc, float* grad, int grad_pitch, double* slots, long long slots_cap,
+                           void* stream) {
+  SN_REQUIRE(slots, "l1_loss_det: null slots");
+  return l1_loss_impl(a, pitch, b_nchw, n, h, w, c, weight, loss_acc, grad, grad_pitch, slots, slots_cap,
+                      (cudaStream_t)stream);
 }
 
 int sn_tap_gemm_simt(const sn_tap_gemm_desc* d, void* stream) {

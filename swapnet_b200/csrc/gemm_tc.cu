@@ -358,7 +358,10 @@ tap_gemm_kernel(const __grid_constant__ TapGemmParams p, const int m_tiles, cons
 // ============================================================================
 // wgrad mode
 // ============================================================================
-template <int NSPLIT, int BN, bool F16>
+// DET: instead of atomically adding its partial into out, CTA (tile, split z) stores it to the plan's workspace
+// det_ws[z][tap][row][col] (plain stores, every valid element of the CTA's tile); wgrad_det_sum_kernel then adds the
+// splits in index order into out.
+template <int NSPLIT, int BN, bool F16, bool DET>
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   using C = Cfg<NSPLIT>;
@@ -500,6 +503,7 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
         const int row = row0 + 8 * h;
         if (row >= p.rows_valid) continue;
         float* orow = p.out + (long long)row * p.s_row;
+        float* wrow = DET ? p.det_ws + (long long)blockIdx.z * p.det_count + (long long)row * p.cols_valid : nullptr;
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
 #pragma unroll
@@ -508,12 +512,17 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
             const float v = acc[4 * i + 2 * h + e];
             if (!grouped) {
               const int col = ncol0 + c;
-              if (c < p.block_n && col < p.cols_valid) atomicAdd(orow + p.tap_off[tap_i] + (long long)col * p.s_col, v);
+              if (c < p.block_n && col < p.cols_valid) {
+                if constexpr (DET) wrow[(long long)tap_i * p.rows_valid * p.cols_valid + col] = v;
+                else atomicAdd(orow + p.tap_off[tap_i] + (long long)col * p.s_col, v);
+              }
             } else {
               const int b = c / ycw;               // which grouped tap this column belongs to
               const int cbase = c - b * ycw;
-              if (b < gsize && cbase < p.cols_valid)
-                atomicAdd(orow + p.tap_off[tap_i + b] + (long long)cbase * p.s_col, v);
+              if (b < gsize && cbase < p.cols_valid) {
+                if constexpr (DET) wrow[(long long)(tap_i + b) * p.rows_valid * p.cols_valid + cbase] = v;
+                else atomicAdd(orow + p.tap_off[tap_i + b] + (long long)cbase * p.s_col, v);
+              }
             }
           }
         }
@@ -522,11 +531,26 @@ wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   }
 }
 
+// out[row*s_row + tap_off[tap] + col*s_col] += sum over the splits z (in order) of det_ws[z][tap][row][col]
+__global__ void __launch_bounds__(256) wgrad_det_sum_kernel(const __grid_constant__ WgradParams p, int ksplit) {
+  const long long rc = (long long)p.rows_valid * p.cols_valid;
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < p.det_count;
+       e += (long long)gridDim.x * blockDim.x) {
+    float s = p.det_ws[e];
+    for (int z = 1; z < ksplit; ++z) s += p.det_ws[(long long)z * p.det_count + e];
+    const int tap = (int)(e / rc);
+    const long long r = e - tap * rc;
+    const int row = (int)(r / p.cols_valid), col = (int)(r - (long long)row * p.cols_valid);
+    p.out[(long long)row * p.s_row + p.tap_off[tap] + (long long)col * p.s_col] += s;
+  }
+}
+
 }  // namespace
 
 // ============================================================================
 // host side
 // ============================================================================
+void sn_count_launch(int n);
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                     const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -826,6 +850,22 @@ int sn_tap_gemm_plan_launch(const TapGemmPlan* plan, cudaStream_t stream) {
   return f16 ? launch_tap_cw<1, true>(plan, stream) : launch_tap_cw<1, false>(plan, stream);
 }
 
+// split-K count: ~3 waves of CTAs on sm_count SMs, at least 8 k-iterations (64-pixel tiles) per CTA; a deterministic
+// plan sizes it for SN_NUM_SMS whatever the device, so that its summation order follows from the shapes alone
+static int wgrad_ksplit(const sn_wgrad_desc* d, int base_ctas, int total, int sm_count) {
+  if (d->deterministic) sm_count = SN_NUM_SMS;
+  int ks = d->ksplit;
+  if (ks <= 0) {
+    ks = (3 * sm_count + base_ctas - 1) / base_ctas;
+    int max_ks = total / 8;
+    if (max_ks < 1) max_ks = 1;
+    if (ks > max_ks) ks = max_ks;
+    if (ks < 1) ks = 1;
+  }
+  if (ks > total) ks = total;
+  return ks;
+}
+
 int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   memset(plan, 0, sizeof(*plan));
   WgradParams& p = plan->p;
@@ -916,29 +956,58 @@ int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count) {
   plan->nsplit = d->nsplit;
   const int base_ctas = p.m_tiles * p.n_tiles * grid_y;
   const int total = p.tiles_w * p.tiles_h * p.tiles_n;
-  int ks = d->ksplit;
-  if (ks <= 0) {  // aim for ~3 waves, at least 8 k-iterations per CTA
-    ks = (3 * sm_count + base_ctas - 1) / base_ctas;
-    int max_ks = total / 8;
-    if (max_ks < 1) max_ks = 1;
-    if (ks > max_ks) ks = max_ks;
-    if (ks < 1) ks = 1;
-  }
-  if (ks > total) ks = total;
+  const int ks = wgrad_ksplit(d, base_ctas, total, sm_count);
   plan->grid = dim3(p.m_tiles * p.n_tiles, grid_y, ks);
+  p.det_ws = nullptr;
+  p.det_count = 0;
+  plan->ws_bytes = 0;
+  if (d->deterministic) {
+    // the finalize kernel writes out[tap_off[t] + ...] from one thread per element: taps must not share outputs
+    for (int t = 0; t < d->ntaps; ++t)
+      for (int u = 0; u < t; ++u)
+        SN_REQUIRE(d->tap_off[t] != d->tap_off[u], "deterministic wgrad: taps %d and %d share tap_off", u, t);
+    p.det_count = (long long)d->ntaps * d->rows_valid * d->cols_valid;
+    plan->ws_bytes = sizeof(float) * (size_t)ks * p.det_count;
+    SN_CHECK_CUDA(cudaMalloc(&p.det_ws, plan->ws_bytes));
+  }
+  return SN_OK;
+}
+
+int sn_wgrad_plan_ksplit(const sn_wgrad_desc* d, int sm_count) {
+  SN_REQUIRE(d && d->ntaps >= 1 && d->ntaps <= SN_MAX_TAPS, "wgrad_ksplit: bad descriptor");
+  int th, tw, nb;
+  pick_patch(d->m_h, d->m_w, 64, &th, &tw, &nb);
+  const int total = ((d->m_w + tw - 1) / tw) * ((d->m_h + th - 1) / th) * ((d->m_n + nb - 1) / nb);
+  const int y_chunk = d->y_chunk ? d->y_chunk : 64;
+  const int grid_y = (y_chunk != 64 && d->ngroups > 0) ? d->ngroups : d->ntaps;
+  const int m_tiles = (d->rows_valid + kBlockM - 1) / kBlockM;
+  const int n_tiles = y_chunk == 64 ? (d->cols_valid + d->block_n - 1) / d->block_n : 1;
+  return wgrad_ksplit(d, m_tiles * n_tiles * grid_y, total, sm_count);
+}
+
+template <int NSPLIT, int BN, bool F16, bool DET>
+static int launch_wgrad_k(const WgradPlan* plan, cudaStream_t stream) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    SN_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<NSPLIT, BN, F16, DET>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<NSPLIT>::kSmemBytes));
+    attr_done = true;
+  }
+  wgrad_gemm_kernel<NSPLIT, BN, F16, DET><<<plan->grid, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p);
+  SN_CHECK_CUDA(cudaGetLastError());
   return SN_OK;
 }
 
 template <int NSPLIT, int BN, bool F16>
 static int launch_wgrad(const WgradPlan* plan, cudaStream_t stream) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    SN_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<NSPLIT, BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       Cfg<NSPLIT>::kSmemBytes));
-    attr_done = true;
-  }
-  wgrad_gemm_kernel<NSPLIT, BN, F16><<<plan->grid, kThreads, Cfg<NSPLIT>::kSmemBytes, stream>>>(plan->p);
+  if (!plan->p.det_ws) return launch_wgrad_k<NSPLIT, BN, F16, false>(plan, stream);
+  const int rc = launch_wgrad_k<NSPLIT, BN, F16, true>(plan, stream);
+  if (rc) return rc;
+  long long g = (plan->p.det_count + 255) / 256;
+  if (g > SN_NUM_SMS * 8) g = SN_NUM_SMS * 8;
+  wgrad_det_sum_kernel<<<(int)g, 256, 0, stream>>>(plan->p, (int)plan->grid.z);
   SN_CHECK_CUDA(cudaGetLastError());
+  sn_count_launch(1);
   return SN_OK;
 }
 

@@ -123,11 +123,12 @@ __device__ __forceinline__ float dp_at(const DyView& d, long long n, int h, int 
 // dW[c*T + t] += sum over this block's pixels of x[px, c] dP[px, t].  block = (C/4 threads.x, rows threads.y):
 // thread = 4 channels, strided over the block's pixel range; T accumulators per channel.  The block first gathers its
 // pixels' dP values (T per pixel) into shared memory, so the main loop is 2 vector loads + T broadcast LDS + 4T FMAs.
+// DET: the block's sums go to slots[blockIdx.x][c*T + t] instead (det_sum_slots adds them in block order).
 constexpr int kWgPix = 256;     // pixels staged per round
-template <int K>
+template <int K, bool DET>
 __global__ void __launch_bounds__(256) to_one_wgrad_kernel(const uint16_t* __restrict__ xhi, const uint16_t* __restrict__ xlo,
                                                            int xpitch, int xfmt, long long npix, int C, const DyView d,
-                                                           float* __restrict__ dW) {
+                                                           float* __restrict__ dW, float* __restrict__ slots) {
   constexpr int T = K * K;
   extern __shared__ float smem[];
   float* dps = smem;                       // [kWgPix][T]
@@ -191,7 +192,8 @@ __global__ void __launch_bounds__(256) to_one_wgrad_kernel(const uint16_t* __res
       for (int t = 0; t < T; ++t) {
         float v = acc[j][t];
         for (int r = 0; r + 1 < (int)blockDim.y; ++r) v += red[r * CT + (c + j) * T + t];
-        atomicAdd(dW + (c + j) * T + t, v);
+        if constexpr (DET) slots[(long long)blockIdx.x * CT + (c + j) * T + t] = v;
+        else atomicAdd(dW + (c + j) * T + t, v);
       }
   }
 }
@@ -266,7 +268,7 @@ int sn_to_one_fwd(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, lo
   if (!attr) {
     SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_fwd_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_dgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_wgrad_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr = true;
   }
   SN_REQUIRE(smem <= 96 * 1024, "to_one_fwd: too many channels (%d)", c);
@@ -278,9 +280,9 @@ int sn_to_one_fwd(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, lo
   return SN_OK;
 }
 
-int sn_to_one_wgrad(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
-                    const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
-                    void* stream) {
+static int to_one_wgrad_impl(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
+                             const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
+                             float* slots, long long slots_cap, cudaStream_t stream) {
   SN_REQUIRE(x_hi && dy_hi && dw && k == 4 && c % 4 == 0 && c <= 1024 && x_pitch % 4 == 0 &&
                  ((uintptr_t)x_hi & 7) == 0 && ((uintptr_t)x_lo & 7) == 0,
              "to_one_wgrad: k = 4, channels %% 4 == 0 and <= 1024");
@@ -295,18 +297,45 @@ int sn_to_one_wgrad(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, 
   if (smem > 48 * 1024) {   // attribute set by the first forward call; set here too for backward-only use
     static bool attr = false;
     if (!attr) {
-      SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_wgrad_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      SN_CHECK_CUDA(cudaFuncSetAttribute(to_one_wgrad_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
       attr = true;
     }
   }
   long long blocks = npix / kWgPix;
   if (blocks > SN_NUM_SMS * 4) blocks = SN_NUM_SMS * 4;
   if (blocks < 1) blocks = 1;
-  to_one_wgrad_kernel<4><<<(int)blocks, dim3(bx, by), smem, (cudaStream_t)stream>>>(
-      (const uint16_t*)x_hi, (const uint16_t*)x_lo, x_pitch, x_fmt, npix, c, d, dw);
+  if (!slots) {
+    to_one_wgrad_kernel<4, false><<<(int)blocks, dim3(bx, by), smem, stream>>>(
+        (const uint16_t*)x_hi, (const uint16_t*)x_lo, x_pitch, x_fmt, npix, c, d, dw, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE(blocks * c * 16 <= slots_cap, "to_one_wgrad_det: %lld slots needed, %lld given", blocks * c * 16, slots_cap);
+  to_one_wgrad_kernel<4, true><<<(int)blocks, dim3(bx, by), smem, stream>>>(
+      (const uint16_t*)x_hi, (const uint16_t*)x_lo, x_pitch, x_fmt, npix, c, d, dw, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, (int)blocks, (long long)c * 16, dw, stream));
   LAUNCH_CHECK();
   return SN_OK;
 }
+
+int sn_to_one_wgrad(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
+                    const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
+                    void* stream) {
+  return to_one_wgrad_impl(x_hi, x_lo, x_pitch, x_fmt, n, h, w, c, dy_hi, dy_lo, dy_pitch, dy_fmt, k, pad, dw, nullptr, 0,
+                           (cudaStream_t)stream);
+}
+
+int sn_to_one_wgrad_det(const void* x_hi, const void* x_lo, int x_pitch, int x_fmt, int n, int h, int w, int c,
+                        const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int k, int pad, float* dw,
+                        float* slots, long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "to_one_wgrad_det: null slots");
+  return to_one_wgrad_impl(x_hi, x_lo, x_pitch, x_fmt, n, h, w, c, dy_hi, dy_lo, dy_pitch, dy_fmt, k, pad, dw, slots,
+                           slots_cap, (cudaStream_t)stream);
+}
+
+long long sn_to_one_wgrad_det_slots(int c) { return (long long)SN_NUM_SMS * 4 * c * 16; }
 
 int sn_to_one_dgrad(const void* dy_hi, const void* dy_lo, int dy_pitch, int dy_fmt, int n, int h, int w, int c,
                     const float* weight, int k, int pad, float* dx, int dx_pitch, void* stream) {

@@ -166,12 +166,13 @@ __global__ void __launch_bounds__(kThreads) relu_pool_bwd_kernel(const float* __
 //   loss += w * sum_c (f_o - f_t)^2;   dx_o = J^T (2 w (f_o - f_t)),  J = d f_o / d x_o
 // NV float4 per lane (C = 128 * NV), or C = 64 with half of the lanes.
 // ---------------------------------------------------------------------------------
-template <int NV>
+// DET: the block's loss sum goes to slots[blockIdx.x] (det_sum_slots adds the blocks in order)
+template <int NV, bool DET>
 __global__ void __launch_bounds__(kThreads) feat_loss_kernel(const float* __restrict__ yo, int po,
                                                               const float* __restrict__ yt, int pt, long long npix,
                                                               int C, double weight, double gscale,
                                                               double* __restrict__ loss_acc,
-                                                              float* __restrict__ dx, int pdx) {
+                                                              float* __restrict__ dx, int pdx, double* slots) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
   const float w = (float)(weight * gscale);
   double local = 0.0;
@@ -231,7 +232,8 @@ __global__ void __launch_bounds__(kThreads) feat_loss_kernel(const float* __rest
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int i = 0; i < wpb; ++i) t += red[i];
-    atomicAdd(loss_acc, t * weight);
+    if constexpr (DET) slots[blockIdx.x] = t * weight;
+    else atomicAdd(loss_acc, t * weight);
   }
 }
 
@@ -243,9 +245,11 @@ constexpr int kGramP = 128;       // pixels per smem tile
 constexpr int kGramMaxR = 96;
 constexpr int kGramAcc = (kGramMaxR * kGramMaxR + kThreads - 1) / kThreads;  // 36
 
+// DET: the block's partial Gram matrix goes to slots[blockIdx.x][R*R] (det_sum_slots adds the blocks in order)
+template <bool DET>
 __global__ void __launch_bounds__(kThreads) gram_kernel(const float* __restrict__ src, long long sn, long long sc,
                                                          long long sp, int C, int R, long long npix,
-                                                         double* __restrict__ G) {
+                                                         double* __restrict__ G, double* __restrict__ slots) {
   extern __shared__ float tile[];   // [R][kGramP + 1]
   constexpr int TP = kGramP + 1;
   float acc[kGramAcc];
@@ -279,7 +283,10 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(const float* __restrict_
 #pragma unroll
   for (int k = 0; k < kGramAcc; ++k) {
     const int idx = k * kThreads + threadIdx.x;
-    if (idx < R * R) atomicAdd(&G[idx], (double)acc[k]);
+    if (idx < R * R) {
+      if constexpr (DET) slots[(long long)blockIdx.x * R * R + idx] = (double)acc[k];
+      else atomicAdd(&G[idx], (double)acc[k]);
+    }
   }
 }
 
@@ -384,45 +391,105 @@ int sn_relu_pool_bwd(const float* y, int y_pitch, const float* g_pool, int gp_pi
   return SN_OK;
 }
 
-int sn_feat_loss_fwd_bwd(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c, double weight,
-                         double gscale, double* loss_acc, float* dx, int pdx, void* stream) {
+}  // extern "C"
+
+template <bool DET>
+static void launch_feat_loss(int blocks, cudaStream_t st, const float* y_out, int po, const float* y_tgt, int pt,
+                             long long npix, int c, double weight, double gscale, double* loss_acc, float* dx, int pdx,
+                             double* slots) {
+  if (c <= 128)
+    feat_loss_kernel<1, DET><<<blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx,
+                                                          pdx, slots);
+  else if (c <= 256)
+    feat_loss_kernel<2, DET><<<blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx,
+                                                          pdx, slots);
+  else
+    feat_loss_kernel<4, DET><<<blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx,
+                                                          pdx, slots);
+}
+
+extern "C" {
+
+static int feat_loss_impl(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c, double weight,
+                          double gscale, double* loss_acc, float* dx, int pdx, double* slots, long long slots_cap,
+                          cudaStream_t st) {
   SN_REQUIRE(y_out && y_tgt && loss_acc && dx, "null pointer");
   SN_REQUIRE(c % 4 == 0 && c <= 512 && po % 4 == 0 && pt % 4 == 0 && pdx % 4 == 0,
              "feat_loss: c multiple of 4 and <= 512, pitches multiples of 4");
   const int wpb = kThreads / 32;
   long long blocks = (npix + wpb - 1) / wpb;
   if (blocks > SN_NUM_SMS * 8) blocks = SN_NUM_SMS * 8;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (c <= 128)
-    feat_loss_kernel<1><<<(int)blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx);
-  else if (c <= 256)
-    feat_loss_kernel<2><<<(int)blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx);
-  else
-    feat_loss_kernel<4><<<(int)blocks, kThreads, 0, st>>>(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx);
+  if (!slots) {
+    launch_feat_loss<false>((int)blocks, st, y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE(blocks <= slots_cap, "feat_loss_det: %lld slots needed, %lld given", blocks, slots_cap);
+  launch_feat_loss<true>((int)blocks, st, y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, (int)blocks, 1, loss_acc, st));
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_feat_loss_fwd_bwd(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c, double weight,
+                         double gscale, double* loss_acc, float* dx, int pdx, void* stream) {
+  return feat_loss_impl(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx, nullptr, 0,
+                        (cudaStream_t)stream);
+}
+
+int sn_feat_loss_fwd_bwd_det(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c,
+                             double weight, double gscale, double* loss_acc, float* dx, int pdx, double* slots,
+                             long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "feat_loss_det: null slots");
+  return feat_loss_impl(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx, slots, slots_cap,
+                        (cudaStream_t)stream);
+}
+
+constexpr int kGramMaxBlocks = 296;
+
+static int gram_impl(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
+                     double* gram, double* slots, long long slots_cap, cudaStream_t st) {
+  SN_REQUIRE(src && gram, "null pointer");
+  const int R = n * c;
+  SN_REQUIRE(R >= 1 && R <= kGramMaxR, "gram: n*c = %d rows, at most %d supported", R, kGramMaxR);
+  SN_CHECK_CUDA(cudaMemsetAsync(gram, 0, sizeof(double) * R * R, st));
+  const size_t smem = (size_t)R * (kGramP + 1) * sizeof(float);
+  static bool attr = false;
+  if (!attr) {
+    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    attr = true;
+  }
+  long long chunks = (npix + kGramP - 1) / kGramP;
+  const int grid = (int)(chunks < kGramMaxBlocks ? chunks : kGramMaxBlocks);
+  if (!slots) {
+    gram_kernel<false><<<grid, kThreads, smem, st>>>(src, s_n, s_c, s_p, c, R, npix, gram, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE((long long)grid * R * R <= slots_cap, "gram_det: %lld slots needed, %lld given", (long long)grid * R * R,
+             slots_cap);
+  gram_kernel<true><<<grid, kThreads, smem, st>>>(src, s_n, s_c, s_p, c, R, npix, gram, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, grid, (long long)R * R, gram, st));
   LAUNCH_CHECK();
   return SN_OK;
 }
 
 int sn_gram(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix, double* gram,
             void* stream) {
-  SN_REQUIRE(src && gram, "null pointer");
-  const int R = n * c;
-  SN_REQUIRE(R >= 1 && R <= kGramMaxR, "gram: n*c = %d rows, at most %d supported", R, kGramMaxR);
-  cudaStream_t st = (cudaStream_t)stream;
-  SN_CHECK_CUDA(cudaMemsetAsync(gram, 0, sizeof(double) * R * R, st));
-  const size_t smem = (size_t)R * (kGramP + 1) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr = true;
-  }
-  long long chunks = (npix + kGramP - 1) / kGramP;
-  const int grid = (int)(chunks < 296 ? chunks : 296);
-  gram_kernel<<<grid, kThreads, smem, st>>>(src, s_n, s_c, s_p, c, R, npix, gram);
-  LAUNCH_CHECK();
-  return SN_OK;
+  return gram_impl(src, s_n, s_c, s_p, n, c, npix, gram, nullptr, 0, (cudaStream_t)stream);
 }
+
+int sn_gram_det(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
+                double* gram, double* slots, long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "gram_det: null slots");
+  return gram_impl(src, s_n, s_c, s_p, n, c, npix, gram, slots, slots_cap, (cudaStream_t)stream);
+}
+
+long long sn_gram_det_slots(int rows) { return (long long)kGramMaxBlocks * rows * rows; }
 
 int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double weight, double* loss_acc, float* m,
                 void* stream) {

@@ -57,6 +57,8 @@ struct alignas(64) WgradParams {
   int ngroups;  // > 0: narrow-Y tap groups (grid.y = group)
   int x_merged, y_merged;   // hi+lo of a 64-channel block in one TMA box (see TapGemmParams)
   short gstart[SN_MAX_TAPS], gsize[SN_MAX_TAPS];
+  float* det_ws;            // deterministic plans: split partials [ksplit][ntaps][rows_valid][cols_valid] (plan-owned)
+  long long det_count;      // ntaps * rows_valid * cols_valid
 };
 
 struct TapGemmPlan {
@@ -69,9 +71,11 @@ struct WgradPlan {
   WgradParams p;
   dim3 grid;
   int nsplit;
+  size_t ws_bytes;          // bytes of p.det_ws
 };
 
 int sn_tap_gemm_plan_init(TapGemmPlan* plan, const sn_tap_gemm_desc* d);
 int sn_tap_gemm_plan_launch(const TapGemmPlan* plan, cudaStream_t stream);
 int sn_wgrad_plan_init(WgradPlan* plan, const sn_wgrad_desc* d, int sm_count);
 int sn_wgrad_plan_launch(const WgradPlan* plan, cudaStream_t stream);
+int sn_wgrad_plan_ksplit(const sn_wgrad_desc* d, int sm_count);

@@ -62,14 +62,15 @@ class Stage:
                   and conv.in_channels <= 1024 and x.c_off % 8 == 0)
         self.layer = (ToOneConvLayer if to_one else ConvLayer)(
             kind, conv.weight.data, None if conv.bias is None else conv.bias.data, x, nsplit=eng.nsplit, act=epi_act,
-            name=name)
+            name=name, det_ws=eng.det_ws_side)
         self.conv = conv
         ly = self.layer
         self.n, self.oh, self.ow, self.cout = ly.n, ly.out_h, ly.out_w, ly.cout
         self.y = y if y is not None else torch.zeros(self.n, self.oh, self.ow, self.cout, device=dev)
-        # InstanceNorm statistics ride on the GEMM epilogue where a tile never spans two images (ConvLayer.fused_stats)
+        # InstanceNorm statistics ride on the GEMM epilogue where a tile never spans two images (ConvLayer.fused_stats),
+        # except in deterministic mode: the epilogue adds them with atomics, ops.plane_stats can add them in order
         self.stats = torch.zeros(self.n, self.cout, 2, dtype=torch.float64, device=dev) if norm else None
-        ly.bind_forward(self.y, stats=self.stats)
+        ly.bind_forward(self.y, stats=None if eng.det_ws is not None else self.stats)
         self.norm, self.act, self.slope, self.drop_p = norm, act, slope, drop_p
         self.out, self.reflect_out, self.residual, self.out_f32 = out, reflect_out, residual, out_f32
         self.plain, self.epi_act, self.need_dx = plain, epi_act, need_dx
@@ -108,13 +109,13 @@ class Stage:
                 ops.bn_eval_stats(self.stats, self.n, self.cout, self.bn)
             else:
                 if not fused:
-                    ops.plane_sums(self.y, self.cout, self.stats)
+                    ops.plane_sums(self.y, self.cout, self.stats, ws=self.eng.det_ws)
                 ops.bn_finalize(self.stats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn)
         elif self.norm:
             if fused:
                 ops.stats_finalize(self.stats, self.n * self.cout, self.oh * self.ow)
             else:
-                ops.plane_stats(self.y, self.cout, self.stats)
+                ops.plane_stats(self.y, self.cout, self.stats, ws=self.eng.det_ws)
         gamma, beta = self._affine()
         p = self.drop_p if self.eng.training else 0.0
         ops.norm_act_fwd(self.y, self.cout, self.stats, self.act, self.slope, p,
@@ -153,7 +154,8 @@ class Stage:
             # the conv's bias gradient (sum of dy over pixels) rides on the pass that writes dy where it can
             bg = None
             if wgrad and self.conv.bias is not None and self.conv.bias.grad is not None and ops.fused_bias_grad_ok(self.cout) \
-                    and self.cout % 4 == 0 and getattr(self.layer, "bgrad_out", None) is not None:
+                    and self.cout % 4 == 0 and getattr(self.layer, "bgrad_out", None) is not None \
+                    and self.eng.det_ws is None:   # the fused bias gradient adds its block sums with atomics
                 bg = self.conv.bias.grad
             bn = bn_grads = None
             if self.bn is not None and not self.plain:
@@ -164,7 +166,7 @@ class Stage:
                              ACT_NONE if self.plain else self.act, self.dy, self.gstats, self.slope, p,
                              _mix_seed(self.eng.seed, self.id), drop_offset=self.drop_offset(),
                              seed_dev=self.eng.seed_dev, stage_id=self.id, bias_grad=bg, bn=bn, bn_groups=self.groups,
-                             bn_train=self.eng.training, bn_grads=bn_grads)
+                             bn_train=self.eng.training, bn_grads=bn_grads, ws=self.eng.det_ws)
             if bg is not None:
                 self._layer_backward(wgrad, bias=False)
                 return
@@ -190,8 +192,15 @@ class Stage:
 class Engine:
     """Common plumbing: stage list, flat gradient buffer, packing."""
 
-    def __init__(self, net: nn.Module, device, nsplit: int, train: bool = True):
+    def __init__(self, net: nn.Module, device, nsplit: int, train: bool = True, deterministic: bool = False):
+        """deterministic: every reduction that spans blocks adds its partial sums in a fixed order instead of with
+        floating-point atomics, so a step gives bit-identical results on every run (DESIGN.md §4)."""
         self.net, self.device, self.nsplit = net, torch.device(device), nsplit
+        self.deterministic = bool(deterministic)
+        # slot workspaces of the deterministic reductions: one for the launching stream, one for the weight-gradient
+        # stream (the two overlap)
+        self.det_ws = ops.DetWorkspace(device) if deterministic else None
+        self.det_ws_side = ops.DetWorkspace(device) if deterministic else None
         self.dual = train   # activation planes carry a bf16-split twin for the weight-gradient GEMMs
         self.stages: List[Stage] = []
         self.training = True
@@ -220,6 +229,14 @@ class Engine:
             done.record(self._wgrad_stream)
             torch.cuda.current_stream(self.device).wait_event(done)
             self._wgrad_pending = False
+
+    def workspace_bytes(self) -> int:
+        """Device bytes of the deterministic mode's workspaces: the slot workspaces (sized by the first step) and the
+        split-K partials of the weight-gradient plans.  0 in the default mode."""
+        if not self.deterministic:
+            return 0
+        plans = [s.layer.wgrad_plan for s in self.stages if getattr(s.layer, "wgrad_plan", None) is not None]
+        return self.det_ws.nbytes + self.det_ws_side.nbytes + sum(p.workspace_bytes for p in plans)
 
     def planes(self, n: int, h: int, w: int, c: int) -> Planes:
         """fp16-split activation operand (+ bf16 twin when training)."""
@@ -268,8 +285,9 @@ class Engine:
 # WarpModule
 # =============================================================================================
 class WarpEngine(Engine):
-    def __init__(self, net: M.WarpModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True):
-        super().__init__(net, device, nsplit, train)
+    def __init__(self, net: M.WarpModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
+                 deterministic: bool = False):
+        super().__init__(net, device, nsplit, train, deterministic)
         assert size % 64 == 0 and size >= 64, "WarpModule needs H = W = 64k (cloth_down6 is H/64)"
         B, S, dev = batch, size, self.device
         self.batch, self.size = B, S
@@ -432,8 +450,9 @@ class PatchGANEngine(Engine):
     separate D calls stacked (the D step's fake and real halves), which matters to batch norm only."""
 
     def __init__(self, net: M.NLayerDiscriminator, batch: int, size: int, device, nsplit: int = 3,
-                 din: Optional[Planes] = None, input_grad: bool = False, train: bool = True, groups: int = 1):
-        super().__init__(net, device, nsplit, train)
+                 din: Optional[Planes] = None, input_grad: bool = False, train: bool = True, groups: int = 1,
+                 deterministic: bool = False):
+        super().__init__(net, device, nsplit, train, deterministic)
         B, S, dev = batch, size, self.device
         self.batch, self.size = B, S
         self.din = din if din is not None else self.planes(B, S, S, L.padc(net.input_nc))
@@ -489,8 +508,9 @@ class TextureEngine(Engine):
       V = dropout?(IN(U(.))) — buffer `cu[j]`, written in place by the producing stages.
     """
 
-    def __init__(self, net: M.TextureModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True):
-        super().__init__(net, device, nsplit, train)
+    def __init__(self, net: M.TextureModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
+                 deterministic: bool = False):
+        super().__init__(net, device, nsplit, train, deterministic)
         B, S = batch, size
         assert S >= 64 and (S & (S - 1)) == 0, "texture stage: power-of-two size >= 64"
         self.batch, self.size = B, S
@@ -643,8 +663,11 @@ class PerceptualEngine:
     """
 
     def __init__(self, net: Optional[M.VGG16Features], batch: int, size: int, device, nsplit: int = 3,
-                 content: bool = True):
+                 content: bool = True, deterministic: bool = False):
+        """deterministic: the content and style sums add their block partials in a fixed order (bit-identical runs);
+        the VGG passes themselves have no cross-block reductions."""
         dev = torch.device(device)
+        self.det_ws = ops.DetWorkspace(dev) if deterministic else None
         self.batch, self.size = batch, size
         self.out = self.tgt = None
         self.gfeat: List[torch.Tensor] = []
@@ -659,6 +682,10 @@ class PerceptualEngine:
         self.gram_o = torch.zeros(r, r, dtype=torch.float64, device=dev)
         self.gram_t = torch.zeros(r, r, dtype=torch.float64, device=dev)
         self.gram_m = torch.zeros(r, r, dtype=torch.float32, device=dev)
+
+    def workspace_bytes(self) -> int:
+        """Device bytes of the deterministic mode's slot workspace (0 in the default mode)."""
+        return 0 if self.det_ws is None else self.det_ws.nbytes
 
     def nominal_macs(self) -> int:
         if self.out is None:
@@ -676,7 +703,7 @@ class PerceptualEngine:
         o.forward()
         for so, st, g in zip(o.taps, t.taps, self.gfeat):
             numel = so.n * so.oh * so.ow * so.cout             # MSELoss: mean over all elements
-            ops.feat_loss_fwd_bwd(so.y, st.y, so.cout, lam / numel, 2.0, acc, g)   # gscale 2 = d(2x-1)/dx
+            ops.feat_loss_fwd_bwd(so.y, st.y, so.cout, lam / numel, 2.0, acc, g, ws=self.det_ws)  # gscale 2: d(2x-1)/dx
         g = None
         ti = len(o.taps) - 1
         for s in reversed(o.chain):
@@ -690,7 +717,7 @@ class PerceptualEngine:
     def style(self, fakes: torch.Tensor, targets: torch.Tensor, lam: float, acc: torch.Tensor,
               grad_accum: torch.Tensor) -> None:
         """acc += lam * 5 * MSE(gram(fakes), gram(targets)); grad_accum [B,S,S,3] += its gradient."""
-        ops.gram(fakes, True, self.gram_o)
-        ops.gram(targets, False, self.gram_t)
+        ops.gram(fakes, True, self.gram_o, ws=self.det_ws)
+        ops.gram(targets, False, self.gram_t, ws=self.det_ws)
         ops.gram_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
         ops.gram_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)

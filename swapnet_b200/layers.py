@@ -19,11 +19,14 @@ from .ops import ACT_NONE, PackedWeights, Planes
 
 class ConvLayer:
     def __init__(self, kind: str, weight: torch.Tensor, bias: Optional[torch.Tensor], x: Planes, *,
-                 nsplit: int = 3, act: int = ACT_NONE, name: str = ""):
+                 nsplit: int = 3, act: int = ACT_NONE, name: str = "", det_ws: Optional[ops.DetWorkspace] = None):
         """x: input operand planes (for 'conv3r' the reflect-padded [h+2, w+2] planes).
-        weight / bias: the torch parameters (torch layout, fp32, on the same device)."""
+        weight / bias: the torch parameters (torch layout, fp32, on the same device).
+        det_ws: deterministic weight and bias gradients (bit-identical runs); the bias-gradient reduction uses this
+        workspace, so it must not be shared with launches that can overlap this layer's backward()."""
         assert kind in L.KINDS
         self.kind, self.name, self.nsplit, self.act = kind, name, nsplit, act
+        self.det_ws = det_ws
         self.weight, self.bias = weight, bias
         self.x = x
         dev = weight.device
@@ -205,7 +208,8 @@ class ConvLayer:
                 assert (ys.c if swap else xs.c) >= 64, f"{self.name}: both wgrad operands are narrow"
             else:
                 swap = cy > cx
-            d = ops.wgrad_desc(xs, ys, ws, out, s_row, s_col, tap_off, cx, cy, swap=swap, nsplit=self.nsplit)
+            d = ops.wgrad_desc(xs, ys, ws, out, s_row, s_col, tap_off, cx, cy, swap=swap, nsplit=self.nsplit,
+                               deterministic=self.det_ws is not None)
             self.wgrad_plan = ops.wgrad_plan(d, keep=(xs.hi, xs.lo, ys.hi, ys.lo, out))
             self.wgrad_plan.tag = ("wgrad", self.name)
         self.bgrad_out = bgrad
@@ -224,7 +228,7 @@ class ConvLayer:
             if self._geff is not None:
                 ops.fold_head_wgrad(self._geff, self.cout, self.cin, self.wgrad_out)
         if wgrad and bias and self.bgrad_out is not None:
-            ops.bias_grad(self.dy, self.cout, self._bscratch, self.bgrad_out)
+            ops.bias_grad(self.dy, self.cout, self._bscratch, self.bgrad_out, ws=self.det_ws)
 
 
 class ToOneConvLayer:
@@ -242,9 +246,10 @@ class ToOneConvLayer:
     K, PAD = 4, 1
 
     def __init__(self, kind: str, weight: torch.Tensor, bias: Optional[torch.Tensor], x: Planes, *,
-                 nsplit: int = 3, act: int = ACT_NONE, name: str = ""):
+                 nsplit: int = 3, act: int = ACT_NONE, name: str = "", det_ws: Optional[ops.DetWorkspace] = None):
         assert kind == "conv4s1" and weight.shape[0] == 1 and tuple(weight.shape[2:]) == (4, 4) and act == ACT_NONE
         self.kind, self.name, self.nsplit, self.act = kind, name, nsplit, act
+        self.det_ws = det_ws
         self.weight, self.bias, self.x = weight, bias, x
         dev = weight.device
         self.cout, self.cin = 1, weight.shape[1]
@@ -290,6 +295,6 @@ class ToOneConvLayer:
         if dgrad and self.dx is not None:
             ops.to_one_dgrad(self.dy, self.weight, self.PAD, self.dx)
         if wgrad and self.wgrad_out is not None:
-            ops.to_one_wgrad(self.x, self.dy, self.PAD, self.wgrad_out)    # the fp16-split planes: no bf16 twin needed
+            ops.to_one_wgrad(self.x, self.dy, self.PAD, self.wgrad_out, ws=self.det_ws)  # fp16-split planes: no twin
         if wgrad and self.bgrad_out is not None:
-            ops.bias_grad(self.dy, 1, self._bscratch, self.bgrad_out)
+            ops.bias_grad(self.dy, 1, self._bscratch, self.bgrad_out, ws=self.det_ws)

@@ -63,6 +63,12 @@ def define_optimizer(module, opt, net: str) -> torch.optim.Optimizer:
     return FusedAdamW(params, flat, lr=lr, weight_decay=wd, betas=(opt.b1, opt.b2), eps=1e-8)
 
 
+def deterministic_mode(opt) -> bool:
+    """--b200_deterministic when given; otherwise torch.use_deterministic_algorithms() as it stands now."""
+    v = getattr(opt, "b200_deterministic", None)
+    return torch.are_deterministic_algorithms_enabled() if v is None else bool(v)
+
+
 class BaseGAN(BaseModel, ABC):
     @staticmethod
     def modify_commandline_options(parser: ArgumentParser, is_train):
@@ -95,6 +101,10 @@ class BaseGAN(BaseModel, ABC):
         parser.add_argument("--b200_graph", type=int, default=1, choices=(0, 1),
                             help="1: replay the training step as a captured CUDA graph (single GPU; after two eager "
                                  "steps per input shape); 0: launch the kernels one by one")
+        parser.add_argument("--b200_deterministic", type=int, default=None, choices=(0, 1),
+                            help="1: bit-identical steps on every run (reductions add their partial sums in a fixed "
+                                 "order instead of with floating-point atomics); 0: the default kernels.  Default: "
+                                 "torch.are_deterministic_algorithms_enabled() when the model is built")
         parser.add_argument("--b200_precision", default="fp32x3", choices=("fp32x3", "bf16"),
                             help="tensor-core arithmetic of the B200 engines: fp32x3 = split-bf16 3-pass "
                                  "(fp32-faithful, parity mode); bf16 = single pass (fast, ~1e-2 relative)")
@@ -103,6 +113,9 @@ class BaseGAN(BaseModel, ABC):
     def __init__(self, opt):
         super().__init__(opt)
         self.nsplit = 1 if getattr(opt, "b200_precision", "fp32x3") == "bf16" else 3
+        self.deterministic = deterministic_mode(opt)
+        # slot workspace of the deterministic loss reductions (launched on the step's stream)
+        self._det_ws = ops.DetWorkspace(self.device) if self.deterministic else None
         self.net_generator = self.define_G().to(self.device)
         M.init_weights(self.net_generator, opt.init_type, opt.init_gain)
         self.model_names = ["generator"]
@@ -229,11 +242,13 @@ class BaseGAN(BaseModel, ABC):
             dn = self.net_discriminator
             # the D step's fake and real halves are two D calls: with batch norm, two sample groups with their own
             # statistics and running-buffer updates (fake first)
-            dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit, groups=2)
+            dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit, groups=2,
+                                            deterministic=self.deterministic)
             dd.alloc_grads()
             dd.bind_backward()
             dg = e["Dg"] = E.PatchGANEngine(dn, batch, size, self.device, self.nsplit,
-                                            din=dd.din.batch_slice(0, batch), input_grad=True)
+                                            din=dd.din.batch_slice(0, batch), input_grad=True,
+                                            deterministic=self.deterministic)
             dg.alloc_grads(share_with=dd)
             dg.bind_backward(wgrad=False)
             e["dpred_d"] = torch.zeros_like(dd.pred)
@@ -295,7 +310,7 @@ class BaseGAN(BaseModel, ABC):
         self.pack_D_inputs(d.din.batch_slice(0, B), d.din.batch_slice(B, B))
         pred = d.forward()
         t = self._targets(0, 2, (1.0, -1.0))                     # order: D_fake, D_real (loss.py:117,121)
-        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 2, t, 0.5, self._acc[0:2], self._dpred_d)
+        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 2, t, 0.5, self._acc[0:2], self._dpred_d, ws=self._det_ws)
         d.backward(self._dpred_d)
         self.allreduce_grads(d)
 
@@ -307,7 +322,8 @@ class BaseGAN(BaseModel, ABC):
         g.pack()
         pred = g.forward()
         t = self._targets(2, 3, (-1.0,))
-        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 1, t, float(self.opt.lambda_gan), self._acc[2:3], self._dpred_g)
+        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 1, t, float(self.opt.lambda_gan), self._acc[2:3], self._dpred_g,
+                             ws=self._det_ws)
         g.backward(self._dpred_g, wgrad=False)
         return g.dx_in
 

@@ -87,13 +87,14 @@ class TextureModel(BaseGAN):
                                norm_type=getattr(self.opt, "norm", "instance"))
 
     def build_generator_engine(self, batch, size):
-        return E.TextureEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train)
+        return E.TextureEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train,
+                               deterministic=self.deterministic)
 
     def _build_engines(self, batch, size):
         e = super()._build_engines(batch, size)
         if self.is_train and (self.lam_content != 0 or self.lam_style != 0):
             e["P"] = E.PerceptualEngine(self.net_vgg, batch, size, self.device, self.nsplit,
-                                        content=self.lam_content != 0)
+                                        content=self.lam_content != 0, deterministic=self.deterministic)
         return e
 
     def ensure_engines(self, batch, size):
@@ -135,7 +136,8 @@ class TextureModel(BaseGAN):
         ct = self.opt.texture_channels
         if not hasattr(self, "_dl1") or self._dl1.shape[0] != B or self._dl1.shape[1] != S:
             self._dl1 = torch.zeros(B, S, S, ct, device=self.device)
-        ops.l1_loss_fwd_bwd(g.fakes, ct, self.targets, float(self.opt.lambda_l1), self._acc[3:4], self._dl1)
+        ops.l1_loss_fwd_bwd(g.fakes, ct, self.targets, float(self.opt.lambda_l1), self._acc[3:4], self._dl1,
+                            ws=self._det_ws)
         srcs = [GradSrc(self._dl1)]
         if self.lam_style != 0:      # 5 x MSE of the raw-image Gram matrices (perceptual.py:58-63): adds into _dl1
             self._eng_P.style(g.fakes, self.targets, self.lam_style, self._acc[5:6], self._dl1)

@@ -66,7 +66,8 @@ class WarpModel(BaseGAN):
         return self.cloth_channels + self.body_channels
 
     def build_generator_engine(self, batch, size):
-        return E.WarpEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train)
+        return E.WarpEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train,
+                            deterministic=self.deterministic)
 
     def set_input(self, input):
         # all H2D copies run on a side stream in the order the step needs them: the body (3 ch) first — the
@@ -124,7 +125,7 @@ class WarpModel(BaseGAN):
         if self.opt.warp_mode == "gan":
             extra.append(GradSrc(self.gan_backward_through_D(), self.body_channels))
         ops.ce_tanh_bwd(g.fakes, self.cloth_channels, self.targets, float(self.opt.lambda_ce), self._acc[3:4], extra,
-                        g.head.dy)
+                        g.head.dy, ws=self._det_ws)
         if self._world > 1:
             from .. import parallel
             avg = parallel.BucketedAverager(g.flat_grad, g.grad_buckets(), scale=False)   # 1/world: in the AdamW kernel

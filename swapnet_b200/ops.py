@@ -97,6 +97,36 @@ class PackedWeights:
         self.hi, self.lo = buf[0], buf[1]
 
 
+class DetWorkspace:
+    """Slot workspace of the deterministic reductions (the *_det entry points): each block stores its partial sums in a
+    slot of its own and a second kernel adds the slots in index order.  Launches on one stream run one after the other
+    and may share a workspace; launches that can overlap (the weight-gradient stream and the launching stream) each need
+    their own.  It grows to the largest request and is sized by the first (eager) step: a CUDA-graph capture that
+    would have to grow it raises."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self._buf: Optional[torch.Tensor] = None
+
+    @property
+    def nbytes(self) -> int:
+        return 0 if self._buf is None else self._buf.numel() * self._buf.element_size()
+
+    def get(self, elems: int, dtype=torch.float64) -> torch.Tensor:
+        """A buffer of at least `elems` elements of dtype (float64 or float32) viewing the workspace."""
+        nb = elems * torch.tensor([], dtype=dtype).element_size()
+        if nb > self.nbytes:
+            if self.device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("DetWorkspace: a CUDA-graph capture cannot grow the workspace; run the step eagerly "
+                                   "first")
+            self._buf = torch.empty((nb + 7) // 8, dtype=torch.float64, device=self.device)
+        return self._buf.view(dtype)
+
+    def slots(self, n: int, c: int) -> torch.Tensor:
+        """float64 slots enough for a deterministic reduction onto [n][c] per-channel values (or a loss)."""
+        return self.get(int(_lib.load().sn_det_slots(n, c)))
+
+
 class Plan:
     """Owns one sn_plan handle (encoded TMA descriptors + launch geometry)."""
 
@@ -104,6 +134,11 @@ class Plan:
         self.handle = handle
         self.tag = tag
         self._keep = list(keep)  # tensors whose addresses are baked into the plan
+
+    @property
+    def workspace_bytes(self) -> int:
+        """Device bytes the plan owns beyond its descriptors (the split partials of a deterministic wgrad plan)."""
+        return int(_lib.load().sn_plan_workspace_bytes(self.handle))
 
     @property
     def has_stats(self) -> bool:
@@ -220,8 +255,10 @@ def tap_gemm_simt(desc: SnTapGemmDesc) -> None:
 
 def wgrad_desc(x: Planes, y: Planes, spec: L.WgradSpec, out: torch.Tensor, s_row: int, s_col: int,
                tap_off: Sequence[int], rows_valid: int, cols_valid: int, *, swap: bool = False,
-               nsplit: int = 3, block_n: Optional[int] = None, ksplit: int = 0) -> SnWgradDesc:
-    """x / y follow the spec orientation; swap=True exchanges the roles (rows <-> cols)."""
+               nsplit: int = 3, block_n: Optional[int] = None, ksplit: int = 0,
+               deterministic: bool = False) -> SnWgradDesc:
+    """x / y follow the spec orientation; swap=True exchanges the roles (rows <-> cols).  deterministic: the split-K
+    partials are added in split order by a second kernel (bit-identical runs), the split count follows from the shapes."""
     xt, yt = spec.xtaps, spec.ytaps
     xp, yp = spec.x_parity, spec.y_parity
     if swap:
@@ -275,7 +312,16 @@ def wgrad_desc(x: Planes, y: Planes, spec: L.WgradSpec, out: torch.Tensor, s_row
         d.block_n = block_n or (128 if cols_valid > 64 else 64)
     d.ksplit = ksplit
     d.nsplit = nsplit
+    d.deterministic = int(deterministic)
     return d
+
+
+def wgrad_ksplit(desc: SnWgradDesc, sm_count: int) -> int:
+    """The split-K count a plan of `desc` gets on a device with sm_count SMs (host logic, no device needed)."""
+    k = _lib.load().sn_wgrad_ksplit(C.byref(desc), sm_count)
+    if k <= 0:
+        check(k)
+    return int(k)
 
 
 def wgrad_plan(desc: SnWgradDesc, keep: Sequence = ()) -> Plan:
@@ -517,11 +563,17 @@ def _pitch(t: torch.Tensor) -> int:
     return p
 
 
-def plane_stats(y: torch.Tensor, c: int, stats: torch.Tensor, eps: float = IN_EPS) -> None:
-    """y fp32 NHWC [n,h,w,pitch]; stats float64 [n, c, 2] <- (mean, rstd)."""
+def plane_stats(y: torch.Tensor, c: int, stats: torch.Tensor, eps: float = IN_EPS,
+                ws: Optional[DetWorkspace] = None) -> None:
+    """y fp32 NHWC [n,h,w,pitch]; stats float64 [n, c, 2] <- (mean, rstd).  ws: deterministic reduction."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)
     assert stats.dtype == torch.float64 and stats.numel() >= n * c * 2
+    if ws is not None:
+        sl = ws.slots(n, c)
+        check(_lib.load().sn_plane_stats_det(y.data_ptr(), pitch, n, h * w, c, eps, stats.data_ptr(), sl.data_ptr(),
+                                             sl.numel(), _stream()))
+        return
     check(_lib.load().sn_plane_stats(y.data_ptr(), pitch, n, h * w, c, eps, stats.data_ptr(), _stream()))
 
 
@@ -530,10 +582,15 @@ def stats_finalize(stats: torch.Tensor, count: int, hw: int, eps: float = IN_EPS
     check(_lib.load().sn_stats_finalize(stats.data_ptr(), count, hw, eps, _stream()))
 
 
-def plane_sums(y: torch.Tensor, c: int, stats: torch.Tensor) -> None:
+def plane_sums(y: torch.Tensor, c: int, stats: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     """y fp32 NHWC [n,h,w,pitch]; stats float64 [n, c, 2] <- (sum, sum of squares) over the plane."""
     n, h, w, _ = y.shape
     assert stats.dtype == torch.float64 and stats.numel() >= n * c * 2
+    if ws is not None:
+        sl = ws.slots(n, c)
+        check(_lib.load().sn_plane_sums_det(y.data_ptr(), _pitch(y), n, h * w, c, stats.data_ptr(), sl.data_ptr(),
+                                            sl.numel(), _stream()))
+        return
     check(_lib.load().sn_plane_sums(y.data_ptr(), _pitch(y), n, h * w, c, stats.data_ptr(), _stream()))
 
 
@@ -619,8 +676,10 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
                  drop_seed: int = 0, drop_offset: int = 0, seed_dev: Optional[torch.Tensor] = None,
                  stage_id: int = 0, bias_grad: Optional[torch.Tensor] = None,
                  bn: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, bn_groups: int = 1, bn_train: bool = True,
-                 bn_grads: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
-    """bias_grad (fp32 [c], c in {256, 512, 1024}): += per-channel sums of the dy written — the bias gradient of the
+                 bn_grads: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                 ws: Optional[DetWorkspace] = None) -> None:
+    """ws: deterministic reduction of the normalisation's gradient statistics (then no fused bias_grad).
+    bias_grad (fp32 [c], c in {256, 512, 1024}): += per-channel sums of the dy written — the bias gradient of the
     conv that produced y — inside the apply pass (see fused_bias_grad_ok).
     bn = (gamma, beta): BatchNorm backward over `bn_groups` sample groups, with batch (bn_train) or running statistics
     in `stats`; bn_grads = (d gamma, d beta) are accumulated (+=) when given."""
@@ -645,6 +704,9 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
         d.bn_groups, d.bn_train = bn_groups, int(bn_train)
         if bn_grads is not None:
             d.gamma_grad, d.beta_grad = bn_grads[0].data_ptr(), bn_grads[1].data_ptr()
+    if ws is not None and stats is not None:
+        sl = ws.slots(n, c)
+        d.det_slots, d.det_slots_cap = sl.data_ptr(), sl.numel()
     check(_lib.load().sn_norm_act_bwd(C.byref(d), _stream()))
 
 
@@ -653,8 +715,14 @@ def fused_bias_grad_ok(c: int) -> bool:
     return c in (256, 512, 1024)
 
 
-def bias_grad(dy: Planes, c: int, scratch: torch.Tensor, db: torch.Tensor) -> None:
+def bias_grad(dy: Planes, c: int, scratch: torch.Tensor, db: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     assert scratch.dtype == torch.float64 and scratch.numel() >= c and db.dtype == torch.float32
+    if ws is not None:
+        sl = ws.slots(1, c)
+        check(_lib.load().sn_bias_grad_det(dy.hi.data_ptr(), dy.lo.data_ptr(), dy.pitch, dy.c_off, dy.fmt,
+                                           dy.n * dy.h * dy.w, c, scratch.data_ptr(), db.data_ptr(), sl.data_ptr(),
+                                           sl.numel(), _stream()))
+        return
     check(_lib.load().sn_bias_grad(dy.hi.data_ptr(), dy.lo.data_ptr(), dy.pitch, dy.c_off, dy.fmt, dy.n * dy.h * dy.w, c,
                                    scratch.data_ptr(), db.data_ptr(), _stream()))
 
@@ -740,7 +808,7 @@ def ce_loss_fwd_bwd(logits: torch.Tensor, c: int, target, weight: float,
 
 
 def ce_tanh_bwd(out: torch.Tensor, c: int, target, weight: float, loss_acc: torch.Tensor,
-                extra: Sequence[GradSrc], dy: Planes) -> None:
+                extra: Sequence[GradSrc], dy: Planes, ws: Optional[DetWorkspace] = None) -> None:
     """Cross entropy on the tanh head's outputs `out` (NHWC [n,h,w,c]) fused with the head's backward:
     dy <- (weight * dCE/d(out) + sum(extra)) * (1 - out^2); loss_acc += weight * CE."""
     n, h, w, pitch = out.shape
@@ -754,9 +822,13 @@ def ce_tanh_bwd(out: torch.Tensor, c: int, target, weight: float, loss_acc: torc
     if extra:
         _fill_srcs(arr, extra)
     assert (dy.n, dy.h, dy.w) == (n, h, w)
-    check(_lib.load().sn_ce_tanh_bwd(out.data_ptr(), pitch, tptr, layout, arr, len(extra), n, h, w, c, weight,
-                                     loss_acc.data_ptr(), dy.hi.data_ptr(), dy.lo.data_ptr(), dy.pitch, dy.c_off,
-                                     dy.fmt, _stream()))
+    args = (out.data_ptr(), pitch, tptr, layout, arr, len(extra), n, h, w, c, weight, loss_acc.data_ptr(),
+            dy.hi.data_ptr(), dy.lo.data_ptr(), dy.pitch, dy.c_off, dy.fmt)
+    if ws is not None:
+        sl = ws.slots(1, 1)
+        check(_lib.load().sn_ce_tanh_bwd_det(*args, sl.data_ptr(), sl.numel(), _stream()))
+        return
+    check(_lib.load().sn_ce_tanh_bwd(*args, _stream()))
 
 
 def bce_logits_fwd_bwd(pred: torch.Tensor, halves: int, t0, t1: float, gscale: float,
@@ -778,7 +850,7 @@ GAN_OBJECTIVES = {"vanilla": GAN_BCE, "lsgan": GAN_MSE, "wgan": GAN_WGAN}
 
 
 def gan_loss_fwd_bwd(objective: int, pred: torch.Tensor, halves: int, t, gscale: float, loss_acc: torch.Tensor,
-                     dpred: Optional[torch.Tensor]) -> None:
+                     dpred: Optional[torch.Tensor], ws: Optional[DetWorkspace] = None) -> None:
     """GANLoss over `halves` (1 or 2) equal consecutive blocks of `pred`, one pass: loss_acc[h] += the unweighted batch
     mean of block h, dpred <- gscale * d(mean)/d(pred).  t holds one scalar per block: the target label of GAN_BCE /
     GAN_MSE, as a device float32 tensor (step-parameter buffer) or a sequence of floats; the sign of GAN_WGAN (+1 for a
@@ -792,13 +864,23 @@ def gan_loss_fwd_bwd(objective: int, pred: torch.Tensor, halves: int, t, gscale:
     else:
         assert len(t) == halves
         t0, t1, tptr = float(t[0]), float(t[-1]), None
-    check(_lib.load().sn_gan_loss_fwd_bwd_dev(objective, pred.data_ptr(), count, halves, t0, t1, tptr, gscale,
-                                              loss_acc.data_ptr(), _ptr(dpred), _stream()))
+    args = (objective, pred.data_ptr(), count, halves, t0, t1, tptr, gscale, loss_acc.data_ptr(), _ptr(dpred))
+    if ws is not None:
+        sl = ws.slots(1, halves)
+        check(_lib.load().sn_gan_loss_fwd_bwd_det(*args, sl.data_ptr(), sl.numel(), _stream()))
+        return
+    check(_lib.load().sn_gan_loss_fwd_bwd_dev(*args, _stream()))
 
 
 def l1_loss_fwd_bwd(a: torch.Tensor, c: int, b_nchw: torch.Tensor, weight: float, loss_acc: torch.Tensor,
-                    grad: torch.Tensor) -> None:
+                    grad: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     n, h, w, pitch = a.shape
+    if ws is not None:
+        sl = ws.slots(1, 1)
+        check(_lib.load().sn_l1_loss_fwd_bwd_det(a.data_ptr(), pitch, b_nchw.data_ptr(), n, h, w, c, weight,
+                                                 loss_acc.data_ptr(), grad.data_ptr(), grad.shape[3], sl.data_ptr(),
+                                                 sl.numel(), _stream()))
+        return
     check(_lib.load().sn_l1_loss_fwd_bwd(a.data_ptr(), pitch, b_nchw.data_ptr(), n, h, w, c, weight,
                                          loss_acc.data_ptr(), grad.data_ptr(), grad.shape[3], _stream()))
 
@@ -879,12 +961,17 @@ def relu_pool_bwd(y: torch.Tensor, c: int, g_pool: Optional[torch.Tensor], g_dir
 
 
 def feat_loss_fwd_bwd(y_out: torch.Tensor, y_tgt: torch.Tensor, c: int, weight: float, gscale: float,
-                      loss_acc: torch.Tensor, dx: torch.Tensor) -> None:
+                      loss_acc: torch.Tensor, dx: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     """loss_acc += weight * sum((f_out - f_tgt)^2), f = relu(y) / (|relu(y)|_2 + 1e-8); dx = gscale * dloss/d relu(y_out)."""
     n, h, w, _ = y_out.shape
     assert y_tgt.shape[:3] == (n, h, w) and dx.shape[:3] == (n, h, w) and loss_acc.dtype == torch.float64
-    check(_lib.load().sn_feat_loss_fwd_bwd(y_out.data_ptr(), _pitch(y_out), y_tgt.data_ptr(), _pitch(y_tgt), n * h * w, c,
-                                           weight, gscale, loss_acc.data_ptr(), dx.data_ptr(), _pitch(dx), _stream()))
+    args = (y_out.data_ptr(), _pitch(y_out), y_tgt.data_ptr(), _pitch(y_tgt), n * h * w, c, weight, gscale,
+            loss_acc.data_ptr(), dx.data_ptr(), _pitch(dx))
+    if ws is not None:
+        sl = ws.slots(1, 1)
+        check(_lib.load().sn_feat_loss_fwd_bwd_det(*args, sl.data_ptr(), sl.numel(), _stream()))
+        return
+    check(_lib.load().sn_feat_loss_fwd_bwd(*args, _stream()))
 
 
 def _gram_strides(x: torch.Tensor, nhwc: bool):
@@ -897,10 +984,15 @@ def _gram_strides(x: torch.Tensor, nhwc: bool):
     return n, c, h * w, c * h * w, h * w, 1
 
 
-def gram(x: torch.Tensor, nhwc: bool, out: torch.Tensor) -> None:
+def gram(x: torch.Tensor, nhwc: bool, out: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     """out [n*c, n*c] (float64) = gram_matrix(x) of perceptual.py:6-10 (rows = (sample, channel))."""
     n, c, npix, sn, sc, sp = _gram_strides(x, nhwc)
     assert out.dtype == torch.float64 and out.numel() == (n * c) ** 2
+    if ws is not None:
+        sl = ws.get(int(_lib.load().sn_gram_det_slots(n * c)))
+        check(_lib.load().sn_gram_det(x.data_ptr(), sn, sc, sp, n, c, npix, out.data_ptr(), sl.data_ptr(), sl.numel(),
+                                      _stream()))
+        return
     check(_lib.load().sn_gram(x.data_ptr(), sn, sc, sp, n, c, npix, out.data_ptr(), _stream()))
 
 
@@ -937,9 +1029,15 @@ def to_one_fwd(x: Planes, weight: torch.Tensor, p: torch.Tensor) -> None:
                                     weight.data_ptr(), 4, p.data_ptr(), _pitch(p), _stream()))
 
 
-def to_one_wgrad(x: Planes, dy: Planes, pad: int, dw: torch.Tensor) -> None:
+def to_one_wgrad(x: Planes, dy: Planes, pad: int, dw: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
     """dw[0,c,kh,kw] += sum_px x[px,c] * dy[px - (kh,kw) + pad] (dy: channel 0 of its planes)."""
     assert dw.is_contiguous() and dw.dtype == torch.float32 and (dy.h, dy.w) == (x.h + 2 * pad - 3, x.w + 2 * pad - 3)
+    if ws is not None:
+        sl = ws.get(int(_lib.load().sn_to_one_wgrad_det_slots(dw.shape[1])), torch.float32)
+        check(_lib.load().sn_to_one_wgrad_det(x.hi_ptr, x.lo_ptr, x.pitch, x.fmt, x.n, x.h, x.w, dw.shape[1], dy.hi_ptr,
+                                              dy.lo_ptr, dy.pitch, dy.fmt, 4, pad, dw.data_ptr(), sl.data_ptr(),
+                                              sl.numel(), _stream()))
+        return
     check(_lib.load().sn_to_one_wgrad(x.hi_ptr, x.lo_ptr, x.pitch, x.fmt, x.n, x.h, x.w, dw.shape[1], dy.hi_ptr,
                                       dy.lo_ptr, dy.pitch, dy.fmt, 4, pad, dw.data_ptr(), _stream()))
 
