@@ -10,6 +10,7 @@
 // All tensors are NHWC fp32 with an explicit pixel pitch; threads map to channels fastest
 // so that every warp touches contiguous 128-B lines.
 #include "common.cuh"
+#include "reflect_pad.h"
 #include "../../include/swapnet_b200.h"
 
 void sn_count_launch(int n);
@@ -777,17 +778,11 @@ __global__ void norm_act_fwd_kernel(const NormActFwdArgs a) {
         } else {
           const int hh = p / a.W, ww = p - hh * a.W;
           const int Hp = a.H + 2, Wp = a.W + 2;
-          int rows[2], cols[2], nr = 1, nc = 1;
-          rows[0] = hh + 1;
-          cols[0] = ww + 1;
-          if (hh == 1) rows[nr++] = 0;
-          if (hh == a.H - 2) rows[nr++] = a.H + 1;
-          if (ww == 1) cols[nc++] = 0;
-          if (ww == a.W - 2) cols[nc++] = a.W + 1;
+          const int nr = reflect_pad1_count(hh, a.H), nc = reflect_pad1_count(ww, a.W);
           for (int i = 0; i < nr; ++i)
             for (int j = 0; j < nc; ++j) {
-              const long long off =
-                  (((long long)n * Hp + rows[i]) * Wp + cols[j]) * a.out_pitch + a.out_coff + c;
+              const long long off = (((long long)n * Hp + reflect_pad1_position(hh, a.H, i)) * Wp +
+                                     reflect_pad1_position(ww, a.W, j)) * a.out_pitch + a.out_coff + c;
               a.hi[off] = h;
               if (a.lo) a.lo[off] = l;
               if (a.hi2) {
@@ -822,16 +817,15 @@ __device__ __forceinline__ float gather_one(const sn_grad_src& s, int n, int h, 
       acc += s.ptr[(((long long)n * H + h) * W + w) * s.pitch + s.c_off + c];
     } else {
       const int Hp = H + 2, Wp = W + 2;
-      int rows[2], cols[2], nr = 1, nc = 1;
-      rows[0] = h + 1;
-      cols[0] = w + 1;
-      if (h == 1) rows[nr++] = 0;
-      if (h == H - 2) rows[nr++] = H + 1;
-      if (w == 1) cols[nc++] = 0;
-      if (w == W - 2) cols[nc++] = W + 1;
+      const int nr = reflect_pad1_count(h, H), nc = reflect_pad1_count(w, W);
+      // kept as loops: the gathers are inlined once per source, and unrolled blocks of up to 3x3 loads raise the
+      // register count of ce_tanh_bwd and of the backward kernels
+#pragma unroll 1
       for (int a = 0; a < nr; ++a)
+#pragma unroll 1
         for (int b = 0; b < nc; ++b)
-          acc += s.ptr[(((long long)n * Hp + rows[a]) * Wp + cols[b]) * s.pitch + s.c_off + c];
+          acc += s.ptr[(((long long)n * Hp + reflect_pad1_position(h, H, a)) * Wp + reflect_pad1_position(w, W, b)) *
+                           s.pitch + s.c_off + c];
     }
   }
   return acc;
@@ -1391,16 +1385,11 @@ __global__ void __launch_bounds__(256, 4) norm_act_fwd_v4_kernel(const NormActFw
       } else {
         const int hh = p / a.W, ww = p - hh * a.W;
         const int Hp = a.H + 2, Wp = a.W + 2;
-        int rows[2], cols[2], nr = 1, nc = 1;
-        rows[0] = hh + 1;
-        cols[0] = ww + 1;
-        if (hh == 1) rows[nr++] = 0;
-        if (hh == a.H - 2) rows[nr++] = a.H + 1;
-        if (ww == 1) cols[nc++] = 0;
-        if (ww == a.W - 2) cols[nc++] = a.W + 1;
+        const int nr = reflect_pad1_count(hh, a.H), nc = reflect_pad1_count(ww, a.W);
         for (int ii = 0; ii < nr; ++ii)
           for (int jj = 0; jj < nc; ++jj) {
-            const long long off = (((long long)n * Hp + rows[ii]) * Wp + cols[jj]) * a.out_pitch + a.out_coff + c;
+            const long long off = (((long long)n * Hp + reflect_pad1_position(hh, a.H, ii)) * Wp +
+                                   reflect_pad1_position(ww, a.W, jj)) * a.out_pitch + a.out_coff + c;
             store_split4(a.hi, a.lo, off, v, a.fmt);
             if (a.hi2) store_split4(a.hi2, a.lo2, off, v, a.fmt2);
           }
@@ -1425,17 +1414,14 @@ __device__ __forceinline__ float4 gather_one4(const sn_grad_src& s, int n, int h
       acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     } else {
       const int Hp = H + 2, Wp = W + 2;
-      int rows[2], cols[2], nr = 1, nc = 1;
-      rows[0] = h + 1;
-      cols[0] = w + 1;
-      if (h == 1) rows[nr++] = 0;
-      if (h == H - 2) rows[nr++] = H + 1;
-      if (w == 1) cols[nc++] = 0;
-      if (w == W - 2) cols[nc++] = W + 1;
+      const int nr = reflect_pad1_count(h, H), nc = reflect_pad1_count(w, W);
+#pragma unroll 1
       for (int a = 0; a < nr; ++a)
+#pragma unroll 1
         for (int b = 0; b < nc; ++b) {
           const float4 v = *reinterpret_cast<const float4*>(
-              s.ptr + (((long long)n * Hp + rows[a]) * Wp + cols[b]) * s.pitch + s.c_off + c);
+              s.ptr + (((long long)n * Hp + reflect_pad1_position(h, H, a)) * Wp + reflect_pad1_position(w, W, b)) *
+                          s.pitch + s.c_off + c);
           acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
         }
     }

@@ -619,8 +619,9 @@ def norm_act_fwd(y: torch.Tensor, c: int, stats: Optional[torch.Tensor], act: in
                  seed_dev: Optional[torch.Tensor] = None, stage_id: int = 0,
                  gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None) -> None:
     """drop_offset: element offset of the keep-mask index (global sample index of the first local sample * h*w*c);
-    seed_dev (uint64/int64[1] on the device) + stage_id: the per-stage seed is derived on the device from the
-    step seed stored there (CUDA-graph replay), drop_seed is then ignored.
+    seed_dev (float32[2] on the device: the 32-bit step seed as its exact 16-bit halves (lo, hi), as
+    set_step_params writes them) + stage_id: the per-stage seed is derived on the device from the step seed
+    stored there (CUDA-graph replay), drop_seed is then ignored.
     gamma, beta (fp32 [c]): BatchNorm's affine, applied before the activation."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)

@@ -23,6 +23,29 @@ def test_planes_views_keep_the_plane_stride():
     assert w.lo.data_ptr() - w.hi.data_ptr() == 2 * 48 * 128
 
 
+def test_reflect_pad_fanout_matches_torch(tmp_path):
+    """csrc/reflect_pad.h compiled for the host: the padded positions of every interior index are exactly the
+    positions torch's ReflectionPad2d(1) fills from it, for axes of 2..9 elements (3 is the axis whose middle
+    index owns both mirrors, three positions)."""
+    import os
+    import sys
+
+    import pytest
+    import torch.nn.functional as F
+
+    sys.path.insert(0, os.path.join(os.path.dirname(__file__), "tools"))
+    import kernel_host_shim
+
+    lib = kernel_host_shim.build_reflect(str(tmp_path))
+    if lib is None:
+        pytest.skip("no g++")
+    for n in range(2, 10):
+        src = F.pad(torch.arange(n, dtype=torch.float64).view(1, 1, n), (1, 1), mode="reflect").view(-1).long()
+        for i in range(n):
+            pos = [lib.position(i, n, k) for k in range(lib.count(i, n))]
+            assert pos[0] == i + 1 and sorted(pos) == (src == i).nonzero().view(-1).tolist(), (n, i, pos)
+
+
 def test_phase_merge_only_for_the_four_parity_phases():
     specs = L.forward_specs("convT4s2", 8, 8)
     m = ops.merge_phase_specs(specs)

@@ -1,5 +1,5 @@
 """Compile the device code of the bit-exact kernels — swapnet_b200/csrc/augment.cu (`build`) and csrc/roi_align.cu
-(`build_roi`) — for the HOST (g++, -ffp-contract=off) so that the CPU suite can run the kernel's own source — index arithmetic, pass ping-pong, the IEEE double/float sequence — against the oracle
+(`build_roi`) — and csrc/reflect_pad.h (`build_reflect`) for the HOST (g++, -ffp-contract=off) so that the CPU suite can run the kernel's own source — index arithmetic, pass ping-pong, the IEEE double/float sequence — against the oracle
 without a GPU.  Test infrastructure only: the CUDA qualifiers and the round-to-nearest intrinsics are defined away,
 blockIdx/threadIdx are globals that a plain loop nest walks.  Nothing in the product uses this."""
 import ctypes as C
@@ -107,4 +107,28 @@ def build_roi(workdir: str):
     lib = C.CDLL(so)
     lib.run_roi.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     lib.run_roi.restype = None
+    return lib
+
+
+REFLECT_DRIVER = r'''
+#include "%s/swapnet_b200/csrc/reflect_pad.h"
+extern "C" int count(int i, int n) { return reflect_pad1_count(i, n); }
+extern "C" int position(int i, int n, int k) { return reflect_pad1_position(i, n, k); }
+'''
+
+
+def build_reflect(workdir: str):
+    """csrc/reflect_pad.h (the ReflectionPad2d(1) fan-out of the norm/activation kernels) for the host ->
+    count(i, n) and position(i, n, k)."""
+    gxx = shutil.which("g++")
+    if gxx is None:
+        return None
+    cpp, so = os.path.join(workdir, "reflect_host.cpp"), os.path.join(workdir, "libreflect_host.so")
+    with open(cpp, "w") as f:
+        f.write(REFLECT_DRIVER % ROOT)
+    subprocess.run([gxx, "-O1", "-shared", "-fPIC", "-o", so, cpp], check=True)
+    lib = C.CDLL(so)
+    lib.count.argtypes = [C.c_int, C.c_int]
+    lib.position.argtypes = [C.c_int, C.c_int, C.c_int]
+    lib.count.restype = lib.position.restype = C.c_int
     return lib
