@@ -339,6 +339,23 @@ int sn_adamw_step_dev(float* p, const float* g, float* m, float* v, long long n,
 void sn_adamw_hyper(double lr, double beta1, double beta2, double eps, double weight_decay, int step, double gscale,
                     float hyper_out[8]);
 
+/* fused AdaBound step over flat fp32 buffers (Luo et al., "Adaptive Gradient Methods with Dynamic Bound of Learning
+ * Rate", ICLR 2019; the update of adabound.AdaBound as optimizers/__init__.py:55-59 builds it, amsbound off), t = step:
+ *   g += wd * p;  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g g;
+ *   p -= clamp(lr sqrt(1 - b2^t) / (1 - b1^t) / (sqrt(v) + eps), lower, upper) * m
+ *   lower = F (1 - 1 / (gamma t + 1)),  upper = F (1 + 1 / (gamma t)),  F = final_lr * lr / base_lr
+ * base_lr is the lr the optimizer was created with (> 0); gamma > 0, final_lr >= 0, step is 1-based. */
+int sn_adabound_step(float* p, const float* g, float* m, float* v, long long n, double lr, double base_lr, double beta1,
+                     double beta2, double eps, double weight_decay, double final_lr, double gamma, int step,
+                     void* stream);
+/* the same update with its scalars read from DEVICE memory (see sn_adamw_step_dev): hyper[8] = { 1 - beta1, 1 - beta2,
+ * eps, wd, lr sqrt(1 - beta2^t) / (1 - beta1^t), lower, upper, gscale }, gscale multiplied into every gradient as it
+ * is read and BEFORE the decay term is added.  sn_adabound_hyper fills the 8 floats on the host. */
+int sn_adabound_step_dev(float* p, const float* g, float* m, float* v, long long n, const float* hyper_dev,
+                         void* stream);
+void sn_adabound_hyper(double lr, double base_lr, double beta1, double beta2, double eps, double weight_decay,
+                       double final_lr, double gamma, int step, double gscale, float hyper_out[8]);
+
 /* per-step scalars of the training step (smooth GAN labels, AdamW scalars, the dropout step seed) live in one small
  * device buffer: dst[0..n) <- vals (n <= 64 floats, passed BY VALUE through the launch, so the host array may be reused
  * immediately); launched once per step ahead of the (possibly graph-replayed) step kernels. */

@@ -165,6 +165,9 @@ SIGNATURES = {
     "sn_adamw_step_dev": (_I, [_VP, _VP, _VP, _VP, _LL, _VP, _VP]),
     "sn_adamw_hyper": (None, [C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _I, C.c_double,
                               C.POINTER(C.c_float)]),
+    "sn_adabound_step": (_I, [_VP, _VP, _VP, _VP, _LL] + [C.c_double] * 8 + [_I, _VP]),
+    "sn_adabound_step_dev": (_I, [_VP, _VP, _VP, _VP, _LL, _VP, _VP]),
+    "sn_adabound_hyper": (None, [C.c_double] * 8 + [_I, C.c_double, C.POINTER(C.c_float)]),
     "sn_set_step_params": (_I, [_VP, C.POINTER(C.c_float), _I, _VP]),
     "sn_bce_logits_fwd_bwd_dev": (_I, [_VP, _LL, _I, _VP, _F, _VP, _VP, _VP]),
     "sn_dropout_mask": (_I, [_ULL, _F, _LL, _VP, _VP]),

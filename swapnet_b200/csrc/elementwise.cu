@@ -1055,6 +1055,54 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
   }
 }
 
+// ---------------------------------------------------------------------------------
+// fused AdaBound over flat fp32 buffers (Luo et al., ICLR 2019; the rule of adabound.AdaBound.step as
+// optimizers/__init__.py:55-59 builds it, amsbound off), with g' = gscale * g:
+//   g' += wd * p  (L2 decay, part of the gradient; skipped when wd == 0)
+//   m += (g' - m)(1 - b1);  v += (g'*g' - v)(1 - b2)
+//   p -= clamp(step_size / (sqrt(v) + eps), lower, upper) * m
+// 1 - b1 and 1 - b2 are passed as rounded on the host: 1.f - (float)0.999 is 1.3e-5 away from 0.001.
+// ---------------------------------------------------------------------------------
+struct AdaBoundHyper { float omb1, omb2, eps, wd, step_size, lower, upper, gscale; };
+__device__ __forceinline__ void adabound_update(float& p, float g, float& m, float& v, const AdaBoundHyper& h) {
+  g *= h.gscale;                     // exact for the power-of-two 1/world of 2, 4, 8 ranks
+  if (h.wd != 0.f) g += h.wd * p;    // after the scaling: 2 ranks of B/2 then decay like 1 rank of B
+  m = m + (g - m) * h.omb1;
+  v = v + (g * g - v) * h.omb2;
+  const float eta = fminf(fmaxf(h.step_size / (sqrtf(v) + h.eps), h.lower), h.upper);
+  p -= eta * m;
+}
+__global__ void __launch_bounds__(256) adabound_kernel(float* __restrict__ p, const float* __restrict__ g,
+                                                       float* __restrict__ m, float* __restrict__ v, long long n,
+                                                       const AdaBoundHyper hv, const float* __restrict__ hyper_dev) {
+  AdaBoundHyper h = hv;
+  if (hyper_dev) {
+    h.omb1 = hyper_dev[0]; h.omb2 = hyper_dev[1]; h.eps = hyper_dev[2]; h.wd = hyper_dev[3];
+    h.step_size = hyper_dev[4]; h.lower = hyper_dev[5]; h.upper = hyper_dev[6]; h.gscale = hyper_dev[7];
+  }
+  const long long n4 = n >> 2;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
+       i += (long long)gridDim.x * blockDim.x) {
+    float4 P = reinterpret_cast<float4*>(p)[i];
+    const float4 G = reinterpret_cast<const float4*>(g)[i];
+    float4 M = reinterpret_cast<float4*>(m)[i];
+    float4 V = reinterpret_cast<float4*>(v)[i];
+    adabound_update(P.x, G.x, M.x, V.x, h);
+    adabound_update(P.y, G.y, M.y, V.y, h);
+    adabound_update(P.z, G.z, M.z, V.z, h);
+    adabound_update(P.w, G.w, M.w, V.w, h);
+    reinterpret_cast<float4*>(p)[i] = P;
+    reinterpret_cast<float4*>(m)[i] = M;
+    reinterpret_cast<float4*>(v)[i] = V;
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {   // tail
+    const long long i = (n4 << 2) + threadIdx.x;
+    float P = p[i], M = m[i], V = v[i];
+    adabound_update(P, g[i], M, V, h);
+    p[i] = P; m[i] = M; v[i] = V;
+  }
+}
+
 __global__ void dropout_mask_kernel(unsigned long long seed, uint32_t thresh, long long count,
                                     uint8_t* out) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count;
@@ -2155,6 +2203,41 @@ int sn_adamw_step_dev(float* p, const float* g, float* m, float* v, long long n,
   SN_REQUIRE(p && g && m && v && n > 0 && hyper_dev, "bad adamw arguments");
   SN_REQUIRE((((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) == 0, "adamw buffers must be 16-B aligned");
   adamw_kernel<<<grid_for(n / 4 + 1), kEwThreads, 0, (cudaStream_t)stream>>>(p, g, m, v, n, AdamHyper{}, hyper_dev);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+void sn_adabound_hyper(double lr, double base_lr, double beta1, double beta2, double eps, double weight_decay,
+                       double final_lr, double gamma, int step, double gscale, float out[8]) {
+  const double bc1 = 1.0 - pow(beta1, (double)step);
+  const double bc2 = 1.0 - pow(beta2, (double)step);
+  const double fin = final_lr * lr / base_lr;   // the bounds follow a scheduler's lr
+  out[0] = (float)(1.0 - beta1); out[1] = (float)(1.0 - beta2); out[2] = (float)eps; out[3] = (float)weight_decay;
+  out[4] = (float)(lr * sqrt(bc2) / bc1);
+  out[5] = (float)(fin * (1.0 - 1.0 / (gamma * step + 1.0)));
+  out[6] = (float)(fin * (1.0 + 1.0 / (gamma * step)));
+  out[7] = (float)gscale;
+}
+
+int sn_adabound_step(float* p, const float* g, float* m, float* v, long long n, double lr, double base_lr, double beta1,
+                     double beta2, double eps, double weight_decay, double final_lr, double gamma, int step,
+                     void* stream) {
+  SN_REQUIRE(p && g && m && v && n > 0 && step >= 1, "bad adabound arguments");
+  SN_REQUIRE(base_lr > 0.0 && gamma > 0.0 && final_lr >= 0.0, "adabound needs base_lr > 0, gamma > 0, final_lr >= 0");
+  SN_REQUIRE((((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) == 0, "adabound buffers must be 16-B aligned");
+  float hp[8];
+  sn_adabound_hyper(lr, base_lr, beta1, beta2, eps, weight_decay, final_lr, gamma, step, 1.0, hp);
+  const AdaBoundHyper h{hp[0], hp[1], hp[2], hp[3], hp[4], hp[5], hp[6], hp[7]};
+  adabound_kernel<<<grid_for(n / 4 + 1), kEwThreads, 0, (cudaStream_t)stream>>>(p, g, m, v, n, h, nullptr);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_adabound_step_dev(float* p, const float* g, float* m, float* v, long long n, const float* hyper_dev,
+                         void* stream) {
+  SN_REQUIRE(p && g && m && v && n > 0 && hyper_dev, "bad adabound arguments");
+  SN_REQUIRE((((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) == 0, "adabound buffers must be 16-B aligned");
+  adabound_kernel<<<grid_for(n / 4 + 1), kEwThreads, 0, (cudaStream_t)stream>>>(p, g, m, v, n, AdaBoundHyper{}, hyper_dev);
   LAUNCH_CHECK();
   return SN_OK;
 }

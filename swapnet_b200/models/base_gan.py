@@ -4,7 +4,8 @@ Keeps the option surface and step order of /root/reference/models/base_gan.py:16
     forward -> zero/backward/step D -> zero/backward/step G        (base_gan.py:194-203)
 with G = a generator engine, D = the conditional PatchGAN (define_D 'basic' / 'n_layers',
 discriminators.py:45-88), GANLoss (loss.py:12-130) for --gan_mode vanilla (BCE-with-logits), lsgan (MSE) and wgan
-(-mean(pred) for real, +mean(pred) for fake) and torch.optim.AdamW exactly as optimizers/__init__.py:37-60 builds it.
+(-mean(pred) for real, +mean(pred) for fake) and torch.optim.AdamW or adabound.AdaBound (--optimizer_G / --optimizer_D,
+chosen per network) exactly as optimizers/__init__.py:37-60 builds them.
 vanilla and lsgan use the reference's smooth labels (loss.py:65-108, including the "fake target drawn from the real
 range" quirk, loss.py:102): three CPU-RNG draws per step, D_fake, D_real, G_gan.  wgan has no target and draws nothing.
 The wgan weight "clamp" of texture_model.py:132-135 (`p.data.clamp(...)`, not in place) leaves D unchanged in the
@@ -19,7 +20,7 @@ What runs differently from the eager reference (results unchanged):
 Unsupported option values raise (there is no eager fallback): --gan_mode wgan-gp / dragan-gp / dragan-lp (the
 gradient penalty needs a second derivative through D), --gan_mode mescheder-r1-gp / mescheder-r2-gp (the reference's
 GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch
-under data parallelism (no cross-rank batch statistics), --optimizer AdaBound.
+under data parallelism (no cross-rank batch statistics).
 """
 from __future__ import annotations
 
@@ -46,20 +47,29 @@ def adam_modifier(parser: ArgumentParser, *_):
     return parser
 
 
+def adabound_modifier(parser: ArgumentParser, *_):
+    """optimizers/__init__.py:31-34: what `--optimizer_G/--optimizer_D AdaBound` reads beyond the Adam flags."""
+    parser = adam_modifier(parser)
+    parser.add_argument("--final_lr", type=float, default=0.1, help="AdaBound final_lr")
+    return parser
+
+
 def define_optimizer(module, opt, net: str) -> torch.optim.Optimizer:
-    """optimizers/__init__.py:37-60 for the AdamW choice, as one fused kernel over flat buffers
-    (swapnet_b200/optim.py); same hyper-parameters, same state_dict layout."""
-    from ..optim import FusedAdamW, flatten_parameters
+    """optimizers/__init__.py:37-60 for both of its choices, AdamW and AdaBound, each as one fused kernel over flat
+    buffers (swapnet_b200/optim.py); same hyper-parameters, same state_dict layout."""
+    from ..optim import FusedAdaBound, FusedAdamW, flatten_parameters
 
     if net not in ("D", "G"):
         raise ValueError(f"net arg must be 'D' or 'G', received {net}")
     choice = getattr(opt, "optimizer_" + net)
-    if choice != "AdamW":
-        raise NotImplementedError(f"optimizer {choice}: only AdamW is available on the B200 plugin")
+    if choice not in ("AdamW", "AdaBound"):
+        raise NotImplementedError(f"optimizer {choice}: only AdamW and AdaBound are available on the B200 plugin")
     lr = opt.d_lr if net == "D" else opt.lr
     wd = opt.d_weight_decay if net == "D" else opt.weight_decay
     params = list(module.parameters())
     flat = flatten_parameters(params)
+    if choice == "AdaBound":
+        return FusedAdaBound(params, flat, lr=lr, weight_decay=wd, betas=(opt.b1, opt.b2), final_lr=opt.final_lr)
     return FusedAdamW(params, flat, lr=lr, weight_decay=wd, betas=(opt.b1, opt.b2), eps=1e-8)
 
 
@@ -159,7 +169,7 @@ class BaseGAN(BaseModel, ABC):
             self._acc = torch.zeros(8, dtype=torch.float64, device=self.device)  # device-side loss sums
             # per-step scalars read by the kernels from DEVICE memory (one tiny launch per step writes them), so that the
             # whole step is a fixed launch sequence a CUDA graph can replay: [0:3] smooth labels (D_fake, D_real, G_gan),
-            # [4:12] AdamW scalars of D, [12:20] of G, [20:22] the dropout step seed as two exact 16-bit halves
+            # [4:12] optimizer scalars of D, [12:20] of G, [20:22] the dropout step seed as two exact 16-bit halves
             self._sp = torch.zeros(32, dtype=torch.float32, device=self.device)
             self._sp_ready = False          # True inside optimize_parameters(): labels were drawn by the step prologue
             self._graphs = {}               # (batch, size, training, input signature) -> captured step
@@ -288,8 +298,8 @@ class BaseGAN(BaseModel, ABC):
         return self._sp[lo:hi]
 
     def allreduce_grads(self, eng) -> None:
-        """Sum over ranks (the 1/world factor is applied by the AdamW kernel as it reads the gradients; code that reads
-        flat_grad directly under DP sees the SUM)."""
+        """Sum over ranks (the 1/world factor is applied by the optimizer kernel as it reads the gradients; code that
+        reads flat_grad directly under DP sees the SUM)."""
         parallel.sum_gradients(eng.flat_grad)
 
     def grad_scale(self) -> float:
@@ -338,7 +348,8 @@ class BaseGAN(BaseModel, ABC):
 
     def _step_prologue(self, optimizers) -> None:
         """Everything of a step that is decided on the host, written to the device with ONE tiny launch: the smooth
-        labels (CPU RNG, reference order; none with wgan), the AdamW scalars of this step, the dropout step seed."""
+        labels (CPU RNG, reference order; none with wgan), both optimizers' scalars of this step, the dropout step
+        seed."""
         vals = [0.0] * 22
         for i in range(self.label_draws()):
             vals[i] = self.draw_label()

@@ -777,6 +777,30 @@ def adamw_step_dev(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.T
                                         hyper_dev.data_ptr(), _stream()))
 
 
+def adabound_step(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, lr: float, base_lr: float,
+                  b1: float, b2: float, eps: float, wd: float, final_lr: float, gamma: float, step: int) -> None:
+    assert p.is_contiguous() and g.is_contiguous() and p.numel() == g.numel() == m.numel() == v.numel()
+    check(_lib.load().sn_adabound_step(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), lr, base_lr,
+                                       b1, b2, eps, wd, final_lr, gamma, step, _stream()))
+
+
+def adabound_hyper(lr: float, base_lr: float, b1: float, b2: float, eps: float, wd: float, final_lr: float,
+                   gamma: float, step: int, gscale: float = 1.0):
+    """The 8 fp32 scalars of sn_adabound_step_dev for optimizer step `step` (1-based), as a list of Python floats."""
+    out = (C.c_float * 8)()
+    _lib.load().sn_adabound_hyper(lr, base_lr, b1, b2, eps, wd, final_lr, gamma, step, gscale, out)
+    return list(out)
+
+
+def adabound_step_dev(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor,
+                      hyper_dev: torch.Tensor) -> None:
+    """AdaBound with its scalars read from device memory (hyper_dev: float32[8] view of the step-parameter buffer)."""
+    assert p.is_contiguous() and g.is_contiguous() and p.numel() == g.numel() == m.numel() == v.numel()
+    assert hyper_dev.dtype == torch.float32 and hyper_dev.numel() >= 8
+    check(_lib.load().sn_adabound_step_dev(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(),
+                                           hyper_dev.data_ptr(), _stream()))
+
+
 def set_step_params(dst: torch.Tensor, values) -> None:
     """dst[:len(values)] <- values (<= 64 floats passed by value through one tiny launch)."""
     n = len(values)
