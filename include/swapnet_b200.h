@@ -82,7 +82,7 @@ typedef struct sn_tap_gemm_desc {
   int b_rows; long long b_k;
   int b_fmt;                             /* SN_FMT_* of the packed weights */
   const float* b_scale;                  /* optional device float[2] = (s, 1/s) written by
-                                            sn_weight_scale: weights were packed as w*s, the
+                                            sn_weight_scale_multi: weights were packed as w*s, the
                                             epilogue multiplies the accumulator by 1/s */
   int m_n, m_h, m_w;                     /* GEMM row grid */
   int ntaps; int k_per_tap;              /* k_per_tap % 64 == 0 (or == a_chunk when narrow) */
@@ -171,20 +171,16 @@ int sn_pack_concat(const float* src0, int layout0, int pitch0, int c0, const flo
                    int c1, int n, int h, int w, int c_fill, void* dst_hi, void* dst_lo, void* dst2_hi, void* dst2_lo,
                    int dst_pitch, int dst_coff, int fmt, int fmt2, void* stream);
 
-/* exact power-of-two scale that brings max|w| into [2^13, 2^14): scale2 <- (s, 1/s). */
-int sn_weight_scale(const float* w, long long count, float* scale2, void* stream);
-
-/* weights -> packed [rows][taps_pitch][k_pad] split planes (taps_pitch >= taps: extra tap slots stay
- * zero, see a_chunk).  Source element (row r, tap t, k) is read at src[r*s_row + k*s_k + t] (taps
- * contiguous, as in torch OIHW / IOHW).  k >= k_real is zero. */
-int sn_pack_weights(const float* src, long long s_row, long long s_k, int rows, int taps, int taps_pitch,
-                    const int* slot_of_tap /* HOST array [taps] or NULL = identity */, int k_real, int k_pad,
-                    void* dst_hi, void* dst_lo, int fmt, const float* scale2, void* stream);
-
-/* multi-tensor variants (one launch per network instead of 3 + 2 per layer).  The item tables live in DEVICE memory and
- * are built once per engine.  sn_weight_scale_multi: scale2 <- (s, 1/s) of every tensor; scratch: 2 * nitems zeroed
- * uint32 (left zeroed).  sn_pack_weights_multi: every item is one sn_pack_weights call; block_begin = running sum of
- * ceil(rows / sn_pack_rows_per_block()) * ceil(k_pad / sn_pack_k_per_block()), total_blocks its end. */
+/* weight packing: torch conv weights -> kernel-layout split planes, a whole network in one launch per entry.  The item
+ * tables live in DEVICE memory and are built once per engine.
+ * sn_weight_scale_multi: scale2 <- (s, 1/s) of every tensor, s the exact power of two that brings max|w| into
+ *   [2^13, 2^14) (1 when max|w| is 0).  Every w 16-byte aligned (float4 loads).  scratch: 2 * nitems zeroed uint32
+ *   (left zeroed).
+ * sn_pack_weights_multi: every item writes packed [rows][taps_pitch][k_pad] split planes (taps_pitch >= taps: extra
+ *   tap slots stay zero, see a_chunk).  Source element (row r, tap t, k) is read at src[r*s_row + k*s_k + t] (taps
+ *   contiguous, as in torch OIHW / IOHW) and written to tap slot slot[t], times scale2[0] when scale2 is not NULL;
+ *   k >= k_real is zero.  taps <= 16, k_pad % 8 == 0, hi / lo 16-byte aligned.  block_begin = running sum of
+ *   ceil(rows / sn_pack_rows_per_block()) * ceil(k_pad / sn_pack_k_per_block()), total_blocks its end. */
 typedef struct sn_scale_item { const float* w; long long count; float* scale2; } sn_scale_item;
 typedef struct sn_pack_item {
   const float* src; long long s_row, s_k;

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — CPU emulator of the two generic contractions of libswapnet_b200
 (tap GEMM / wgrad GEMM, csrc/gemm_tc.cu) plus torch restatements of the weight packers
-(csrc/elementwise.cu pack_weights / pack_head_weights / fold_head_wgrad).
+(csrc/elementwise.cu pack_weights_multi / pack_head_weights / fold_head_wgrad).
 
 Used by tests/ to (a) prove on the CPU that swapnet_b200/lowering.py maps every reference conv
 layer (modules/layers.py:15,31,131-138; swapnet_modules.py:85-90; discriminators.py:111-131)

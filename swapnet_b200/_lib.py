@@ -145,8 +145,6 @@ SIGNATURES = {
     "sn_bn_eval_stats": (_I, [_VP, _I, _I, _VP, _VP, _F, _VP]),
     "sn_pack_planes": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_pack_concat": (_I, [_VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
-    "sn_weight_scale": (_I, [_VP, _LL, _VP, _VP]),
-    "sn_pack_weights": (_I, [_VP, _LL, _LL, _I, _I, _I, C.POINTER(C.c_int), _I, _I, _VP, _VP, _I, _VP, _VP]),
     "sn_pack_head_weights": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _VP, _VP]),
     "sn_weight_scale_multi": (_I, [_VP, _I, _VP, _VP]),
     "sn_pack_weights_multi": (_I, [_VP, _I, _I, _I, _VP]),

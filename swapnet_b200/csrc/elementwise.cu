@@ -242,34 +242,6 @@ __global__ void __launch_bounds__(256) pack_concat_direct_kernel(const PackConca
 }
 
 // ---------------------------------------------------------------------------------
-// pack_weights: dst[r][t][k] <- src[r*s_row + k*s_k + t]
-// ---------------------------------------------------------------------------------
-struct TapSlots { int slot[64]; };   // packed slot of each source tap
-__global__ void pack_weights_kernel(const TapSlots ts, const float* __restrict__ src, long long s_row, long long s_k,
-                                    int taps, int taps_pitch, int k_real, int k_pad, uint16_t* __restrict__ hi,
-                                    uint16_t* __restrict__ lo, int fmt, const float* __restrict__ scale2) {
-  extern __shared__ float tile[];  // [32][taps + 1]
-  const float sc = scale2 ? scale2[0] : 1.f;
-  const int r = blockIdx.y;
-  const int k0 = blockIdx.x * 32;
-  const int T1 = taps + 1;
-  for (int i = threadIdx.x; i < 32 * taps; i += blockDim.x) {
-    const int kk = i / taps, t = i % taps;
-    float v = 0.f;
-    if (k0 + kk < k_real) v = src[r * s_row + (long long)(k0 + kk) * s_k + t];
-    tile[kk * T1 + t] = v;
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 32 * taps; i += blockDim.x) {
-    const int t = i / 32, kk = i % 32;
-    if (k0 + kk < k_pad) {
-      const long long off = ((long long)r * taps_pitch + ts.slot[t]) * k_pad + k0 + kk;
-      store_split(hi, lo, off, tile[kk * T1 + t] * sc, fmt);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------
 // head weights: nearest-x2 upsample + ZeroPad2d((1,0,1,0)) + Conv2d(k=4, p=1) seen from an
 // output pixel o = 2m + par reads up-sampled u = o + k - 2, k = 0..3, i.e. source s = u >> 1:
 //   par 0: k=0,1 -> m-1 ; k=2,3 -> m          (2 effective taps: d = -1, 0)
@@ -371,32 +343,9 @@ __global__ void fold_head_wgrad_kernel(const float* __restrict__ geff, int cout,
 }
 
 // ---------------------------------------------------------------------------------
-// per-tensor power-of-two weight scale (fp16-split operands): s = 2^k with max|w|*s in [2^13, 2^14)
-// ---------------------------------------------------------------------------------
-__global__ void absmax_kernel(const float* __restrict__ w, long long count, unsigned int* out) {
-  float m = 0.f;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count;
-       i += (long long)gridDim.x * blockDim.x)
-    m = fmaxf(m, fabsf(w[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));  // non-negative floats order as uints
-}
-__global__ void weight_scale_finalize_kernel(const unsigned int* amax, float* scale2) {
-  const float m = __uint_as_float(*amax);
-  float s = 1.f;
-  if (m > 0.f && isfinite(m)) {
-    int e;
-    frexpf(m, &e);          // m = f * 2^e, f in [0.5, 1)
-    s = ldexpf(1.f, 14 - e);  // m * s in [2^13, 2^14)
-  }
-  scale2[0] = s;
-  scale2[1] = 1.f / s;
-}
-
-// ---------------------------------------------------------------------------------
-// multi-tensor variants: ONE launch computes the power-of-two scales of every weight tensor of a network, ONE launch
-// writes every packed copy (forward and input-gradient layouts) — instead of 3 + 2 launches per layer per step.
+// weight packing: ONE launch computes the power-of-two scales of every weight tensor of a network (fp16-split
+// operands: s = 2^k with max|w|*s in [2^13, 2^14)), ONE launch writes every packed copy (forward and input-gradient
+// layouts: dst[r][slot[t]][k] <- src[r*s_row + k*s_k + t] * s).
 // ---------------------------------------------------------------------------------
 // grid (blocks per tensor, tensors).  scratch[2t] = max |w| bits, scratch[2t+1] = blocks done; the last block of a
 // tensor finalises its scale and resets both words (the buffer is zero again when the launch retires).
@@ -1763,24 +1712,6 @@ int sn_pack_concat(const float* src0, int layout0, int pitch0, int c0, const flo
   return SN_OK;
 }
 
-int sn_pack_weights(const float* src, long long s_row, long long s_k, int rows, int taps, int taps_pitch,
-                    const int* slot_of_tap, int k_real, int k_pad, void* dst_hi, void* dst_lo, int fmt,
-                    const float* scale2, void* stream) {
-  SN_REQUIRE(src && dst_hi, "null pointer");
-  TapSlots ts;
-  for (int t = 0; t < taps && t < 64; ++t) {
-    ts.slot[t] = slot_of_tap ? slot_of_tap[t] : t;
-    SN_REQUIRE(ts.slot[t] >= 0 && ts.slot[t] < taps_pitch, "pack_weights: slot_of_tap[%d] out of range", t);
-  }
-  SN_REQUIRE(taps >= 1 && taps <= 64 && k_pad >= k_real && taps_pitch >= taps, "bad pack_weights shape");
-  dim3 grid((k_pad + 31) / 32, rows);
-  size_t smem = (size_t)32 * (taps + 1) * sizeof(float);
-  pack_weights_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(
-      ts, src, s_row, s_k, taps, taps_pitch, k_real, k_pad, (uint16_t*)dst_hi, (uint16_t*)dst_lo, fmt, scale2);
-  LAUNCH_CHECK();
-  return SN_OK;
-}
-
 int sn_pack_head_weights(const float* src, int cout, int cin, int rows_pad, int k_pad, int dgrad, int taps_pitch,
                          void* dst_hi, void* dst_lo, int fmt, const float* scale2, void* stream) {
   SN_REQUIRE(src && dst_hi, "null pointer");
@@ -1797,19 +1728,6 @@ int sn_pack_head_stacked(const float* src, int cout, int cin, int slot, int k_pa
   SN_REQUIRE(src && dst_hi && slot >= cout && k_pad >= cin, "bad stacked head pack shape");
   pack_head_stacked_kernel<<<grid_for((long long)4 * slot * 9 * k_pad), kEwThreads, 0, (cudaStream_t)stream>>>(
       src, cout, cin, slot, k_pad, (uint16_t*)dst_hi, (uint16_t*)dst_lo, fmt, scale2);
-  LAUNCH_CHECK();
-  return SN_OK;
-}
-
-int sn_weight_scale(const float* w, long long count, float* scale2, void* stream) {
-  SN_REQUIRE(w && scale2, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  // scale2[1] doubles as the atomicMax scratch before the finalize kernel overwrites it
-  unsigned int* scratch = reinterpret_cast<unsigned int*>(scale2 + 1);
-  SN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(unsigned int), st));
-  absmax_kernel<<<grid_for(count), kEwThreads, 0, st>>>(w, count, scratch);
-  LAUNCH_CHECK();
-  weight_scale_finalize_kernel<<<1, 1, 0, st>>>(scratch, scale2);
   LAUNCH_CHECK();
   return SN_OK;
 }

@@ -135,19 +135,13 @@ class ConvLayer:
             ops.pack_head_weights(self.weight, 0, self.dy.c, True, self.wd)
 
     def pack(self) -> None:
-        """Re-pack the (updated) torch weights into the kernel layouts (per-layer launches: tests, single layers)."""
-        ops.weight_scale(self.weight, self.wscale)
-        if self.kind == "head":
-            if self.stacked:
-                ops.pack_head_stacked(self.weight, L.HEAD_SLOT, self.k_pad, self.wp)
-            else:
-                ops.pack_head_weights(self.weight, self.rows_pad, self.k_pad, False, self.wp)
-            if self.wd is not None and self.dgrad_plans:
-                ops.pack_head_weights(self.weight, 0, self.dy.c, True, self.wd)
-        else:
-            ops.pack_weights(self.weight, self.kind, False, self.k_pad, self.wp)
-            if self.wd is not None and self.dgrad_plans:
-                ops.pack_weights(self.weight, self.kind, True, self.dy.c, self.wd)
+        """Re-pack the (updated) torch weights into the kernel layouts: the steps of Engine.pack() with a table of this
+        layer alone (tests, single layers).  The table is rebuilt on every call: bind_backward() adds a pack."""
+        table = ops.PackTable(self.weight.device)
+        extra = self.register_packs(table)
+        table.run()
+        if extra:
+            self.pack_extra()
 
     def forward(self) -> None:
         for p in self.fwd_plans:

@@ -86,7 +86,7 @@ def phase_major_slots() -> List[int]:
 
 
 def pack_slots(kind: str, dgrad: bool) -> List[int]:
-    """slot_of_tap for sn_pack_weights (identity except for the 4-phase structures)."""
+    """Packed tap slot of each torch tap for sn_pack_weights_multi (identity except for the 4-phase structures)."""
     if (kind == "convT4s2" and not dgrad) or (kind == "conv4s2" and dgrad):
         return phase_major_slots()
     return list(range(ntaps(kind)))
@@ -260,10 +260,10 @@ def wgrad_specs(kind: str, h: int, w: int) -> List[WgradSpec]:
 
 # ------------------------------------------------------------------------------------------
 # weight layouts.  torch layouts: conv OIHW [cout][cin][k][k]; convT IOHW [cin][cout][k][k].
-# pack_weights reads src[row*s_row + k*s_k + tap].
+# pack_weights_multi reads src[row*s_row + k*s_k + tap].
 # ------------------------------------------------------------------------------------------
 def pack_strides(kind: str, cin: int, cout: int, dgrad: bool) -> Tuple[int, int, int, int]:
-    """-> (s_row, s_k, rows, k_real) for sn_pack_weights (not for 'head')."""
+    """-> (s_row, s_k, rows, k_real) for sn_pack_weights_multi (not for 'head')."""
     t = ntaps(kind)
     if kind == "convT4s2":
         if not dgrad:  # rows = co, k = ci

@@ -86,7 +86,7 @@ class Planes:
 
 class PackedWeights:
     """[rows][k_total] split 16-bit weight matrix (K contiguous), fp16-split with an exact
-    power-of-two scale (`scale` = device (s, 1/s), set by weight_scale())."""
+    power-of-two scale (`scale` = device (s, 1/s), set by a PackTable scale item)."""
 
     def __init__(self, rows: int, k_total: int, device, scale: Optional[torch.Tensor] = None, fmt: int = FMT_F16):
         self.rows, self.k_total = rows, k_total
@@ -436,27 +436,6 @@ def pack_concat(srcs, dst: Planes) -> None:
                                      dst.pitch, dst.c_off, dst.fmt, FMT_BF16 if tw is None else tw.fmt, _stream()))
 
 
-def weight_scale(weight: torch.Tensor, scale: torch.Tensor) -> None:
-    """scale <- (s, 1/s), s = 2^k with max|w| * s in [2^13, 2^14) (device side, no sync)."""
-    check(_lib.load().sn_weight_scale(weight.data_ptr(), weight.numel(), scale.data_ptr(), _stream()))
-
-
-def pack_weights(weight: torch.Tensor, kind: str, dgrad: bool, k_pad: int, dst: PackedWeights) -> None:
-    assert weight.is_contiguous() and weight.dtype == torch.float32
-    if kind == "convT4s2":
-        cin, cout = weight.shape[0], weight.shape[1]
-    else:
-        cout, cin = weight.shape[0], weight.shape[1]
-    s_row, s_k, rows, k_real = L.pack_strides(kind, cin, cout, dgrad)
-    t = L.ntaps(kind)
-    assert dst.rows >= rows and dst.k_total >= t * k_pad and k_pad >= k_real and dst.k_total % k_pad == 0
-    slots = (C.c_int * t)(*L.pack_slots(kind, dgrad))
-    check(_lib.load().sn_pack_weights(weight.data_ptr(), s_row, s_k, rows, t, dst.k_total // k_pad, slots, k_real,
-                                      k_pad, dst.hi.data_ptr(),
-                                      dst.lo.data_ptr(), dst.fmt, None if dst.scale is None else dst.scale.data_ptr(),
-                                      _stream()))
-
-
 class PackTable:
     """All weight-scale and pack launches of one network as TWO launches (sn_weight_scale_multi,
     sn_pack_weights_multi): layers register their tensors once, the item tables live in device memory."""
@@ -467,14 +446,17 @@ class PackTable:
         self._dev = None
 
     def add_scale(self, weight: torch.Tensor, scale: torch.Tensor) -> None:
+        """scale <- (s, 1/s) at every run(), s = 2^k with max|w| * s in [2^13, 2^14)."""
         assert weight.is_contiguous() and weight.dtype == torch.float32 and self._dev is None
+        assert weight.data_ptr() % 16 == 0, "weight_scale_multi reads float4: the weight must be 16-byte aligned"
         it = _lib.SnScaleItem()
         it.w, it.count, it.scale2 = weight.data_ptr(), weight.numel(), scale.data_ptr()
         self._scales.append(it)
         self._keep += [weight, scale]
 
     def add_pack(self, weight: torch.Tensor, kind: str, dgrad: bool, k_pad: int, dst: PackedWeights) -> None:
-        """Same arguments as pack_weights()."""
+        """dst <- the torch-layout weight of a `kind` conv in its forward (dgrad=False) or input-gradient kernel
+        layout, K padded to k_pad, scaled by dst.scale[0] when dst has a scale."""
         assert weight.is_contiguous() and weight.dtype == torch.float32 and self._dev is None
         if kind == "convT4s2":
             cin, cout = weight.shape[0], weight.shape[1]

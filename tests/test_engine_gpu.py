@@ -768,35 +768,122 @@ def test_graph_replayed_steps_match_eager_steps():
     record("graph_vs_eager_5_steps", f"max |dW| {(wg - we).abs().max().item():.2e}; launches/step graph {lg} eager {le}")
 
 
-def test_pack_table_equals_per_layer_packs():
-    """Engine.pack(): one multi-tensor scale launch + one multi-tensor pack launch must write exactly the bytes the
-    per-layer sn_weight_scale / sn_pack_weights launches write (forward and input-gradient layouts, all conv kinds)."""
+def packed_ref(layer, dgrad):
+    """Unscaled fp32 contents of layer.wd (dgrad) or layer.wp: the host restatements of the packed layouts in
+    oracle/emulate.py, zero in the padding rows and tap slots."""
+    from oracle import emulate as EM
+    from swapnet_b200 import lowering as L
+
+    w = layer.weight.detach().cpu()
+    pw, k_pad = (layer.wd, layer.dy.c) if dgrad else (layer.wp, layer.k_pad)
+    if layer.kind != "head":
+        m = EM.pack_weights_ref(w, layer.kind, dgrad, k_pad)
+    elif dgrad:
+        m = EM.pack_head_ref(w, 0, k_pad, True)
+    elif layer.stacked:       # [phase * HEAD_SLOT + co][3 x 3 shifts][ci], zero where a phase has no tap at a shift
+        eff, S = EM.head_eff_weights(w), L.HEAD_SLOT
+        m = w.new_zeros(4 * S, 9, k_pad)
+        for p in range(4):
+            for ey in range(L.head_neff(p >> 1)):
+                for ex in range(L.head_neff(p & 1)):
+                    m[p * S:p * S + layer.cout, ey * 3 + ex, :layer.cin] = \
+                        eff[:, L.HEAD_PHASE_OFF[p] + ey * L.head_neff(p & 1) + ex]
+        m = m.reshape(4 * S, 9 * k_pad)
+    else:                     # the four per-phase matrices one after the other
+        m = torch.cat([x.reshape(-1) for x in EM.pack_head_ref(w, layer.rows_pad, k_pad, False)]).view(pw.rows, -1)
+    out = torch.zeros(pw.rows, pw.k_total)
+    out[:m.shape[0], :m.shape[1]] = m
+    return out
+
+
+def check_layer_packs(layer):
+    """layer.wscale and the layer's packed copies, bit for bit against the host reference: s = 2^(14 - e) with
+    max|w| = f * 2^e, f in [0.5, 1) (1 for an all-zero weight); fp16-split packs hold the weights times s, saturated
+    at the fp16 range, bf16-split packs the weights themselves; hi = rn16(v), lo = rn16(v - hi) (split16 in
+    csrc/common.cuh)."""
+    import math
+
+    from swapnet_b200 import ops
+
+    m = layer.weight.detach().abs().max().item()
+    s = 1.0 if m == 0 else 2.0 ** (14 - math.frexp(m)[1])
+    assert torch.equal(layer.wscale.cpu(), torch.tensor([s, 1 / s])), (layer.name, layer.wscale, s)
+    for dgrad, pw in ((False, layer.wp), (True, layer.wd)):
+        if dgrad and not layer.dgrad_plans:
+            continue
+        v = packed_ref(layer, dgrad)
+        if pw.fmt == ops.FMT_F16:
+            v, t = (v * (1.0 if pw.scale is None else s)).clamp(-65504, 65504), torch.float16
+        else:
+            assert pw.scale is None
+            t = torch.bfloat16
+        hi = v.to(t)
+        lo = (v - hi.float()).to(t)
+        assert torch.equal(pw.hi.cpu().view(torch.int16), hi.view(torch.int16)), (layer.name, dgrad, "hi")
+        assert torch.equal(pw.lo.cpu().view(torch.int16), lo.view(torch.int16)), (layer.name, dgrad, "lo")
+
+
+def test_engine_pack_equals_host_reference():
+    """Engine.pack() (one multi-tensor scale launch, one multi-tensor pack launch, the head's effective-tap packs)
+    writes exactly the scales and split planes of the host reference: forward and input-gradient layouts of every
+    conv layer of the warp generator and the PatchGAN."""
     from swapnet_b200 import engine as E
+    from swapnet_b200.layers import ConvLayer
 
     G, D = make_nets()
     for net, mk in ((G, lambda n: E.WarpEngine(n, 1, 64, dev())), (D, lambda n: E.PatchGANEngine(n, 2, 64, dev(), input_grad=True))):
         eng = mk(net.to(dev()))
         eng.alloc_grads()
         eng.bind_backward()
-        bufs = []
-        for st in eng.stages:
-            st.layer.pack()                                   # per-layer launches
-            for pw in (getattr(st.layer, "wp", None), getattr(st.layer, "wd", None)):
-                if pw is not None:
-                    bufs.append((st.name, pw, pw.hi.clone(), pw.lo.clone()))
-            if hasattr(st.layer, "wscale"):
-                bufs.append((st.name + ".scale", st.layer.wscale, st.layer.wscale.clone(), None))
-        for _, pw, _, _ in bufs:
-            if hasattr(pw, "hi"):
-                pw.hi.zero_()
-                pw.lo.zero_()
-            else:
-                pw.zero_()
-        eng.pack()                                            # the table
-        eng.pack()                                            # (scratch words self-reset: a second run is identical)
-        torch.cuda.synchronize()
-        for name, pw, hi, lo in bufs:
-            if lo is None:
-                assert torch.equal(pw, hi), name
-            else:
-                assert torch.equal(pw.hi, hi) and torch.equal(pw.lo, lo), name
+        layers = [st.layer for st in eng.stages if isinstance(st.layer, ConvLayer)]
+        for _ in range(2):    # the scale launch resets its scratch words: a second run on cleared outputs is identical
+            for ly in layers:
+                ly.wscale.zero_()
+                for pw in (ly.wp, ly.wd):
+                    if pw is not None:
+                        pw.hi.zero_()
+                        pw.lo.zero_()
+            eng.pack()
+            torch.cuda.synchronize()
+            for ly in layers:
+                check_layer_packs(ly)
+
+
+# kind, cin, cout, input channels (forward K), gradient channels (input-gradient K; None: no input gradient)
+PACK_EDGE_CASES = {
+    "tail": ("conv3z", 3, 3, 16, None),        # 81 floats: the largest |w| is the last, after the 20 float4 loads
+    "zero": ("conv4s2", 19, 64, 32, 64),       # all-zero weight: scale 1, zero planes
+    "pow2": ("convT4s2", 64, 3, 64, 16),       # max |w| = 2^-1 exactly (frexp boundary: max|w| * s = 2^13)
+    "head27": ("head", 64, 27, 64, None),      # more outputs than HEAD_SLOT: the unstacked forward pack
+}
+
+
+@pytest.mark.parametrize("case", sorted(PACK_EDGE_CASES))
+def test_layer_pack_edges(case):
+    """ConvLayer.pack() (a pack table of one layer) on what the engines' weights do not show: a count that is not a
+    multiple of 4, all zeros, a power-of-two maximum, K padded to 16 and 32 channels, the unstacked head."""
+    from swapnet_b200 import lowering as L
+    from swapnet_b200 import ops
+    from swapnet_b200.layers import ConvLayer
+
+    kind, cin, cout, xc, dyc = PACK_EDGE_CASES[case]
+    n, h, w = 1, 16, 16
+    k = 3 if kind == "conv3z" else 4
+    g = torch.Generator().manual_seed(5)
+    wt = torch.randn((cin, cout, k, k) if kind == "convT4s2" else (cout, cin, k, k), generator=g) * 0.1
+    if case == "tail":
+        wt.view(-1)[-1] = -3 * wt.abs().max()
+    elif case == "zero":
+        wt.zero_()
+    elif case == "pow2":
+        wt = wt.clamp(-0.25, 0.25)
+        wt.view(-1)[100] = -0.5
+    layer = ConvLayer(kind, wt.to(dev()), None, ops.Planes(n, h, w, xc, dev()), name=case)
+    if dyc is not None:
+        oh, ow = L.out_hw(kind, h, w)
+        layer.bind_backward(ops.Planes(n, oh, ow, dyc, dev(), fmt=ops.FMT_BF16),
+                            torch.zeros(n, h, w, cin, device=dev()), None)
+        assert layer.dgrad_plans
+    layer.pack()
+    torch.cuda.synchronize()
+    check_layer_packs(layer)

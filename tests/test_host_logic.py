@@ -23,6 +23,18 @@ def test_planes_views_keep_the_plane_stride():
     assert w.lo.data_ptr() - w.hi.data_ptr() == 2 * 48 * 128
 
 
+def test_pack_table_refuses_a_misaligned_weight():
+    """The scale kernel reads weights as float4 (csrc/elementwise.cu weight_scale_multi_kernel): a weight that does not
+    start on a 16-byte boundary is refused when it is registered, not read misaligned on the device."""
+    import pytest
+
+    table = ops.PackTable("cpu")
+    flat = torch.zeros(20)
+    table.add_scale(flat[4:13], torch.ones(2))        # 16-byte aligned, 9 floats: the tail is the kernel's business
+    with pytest.raises(AssertionError, match="16-byte aligned"):
+        table.add_scale(flat[1:9], torch.ones(2))
+
+
 def test_reflect_pad_fanout_matches_torch(tmp_path):
     """csrc/reflect_pad.h compiled for the host: the padded positions of every interior index are exactly the
     positions torch's ReflectionPad2d(1) fills from it, for axes of 2..9 elements (3 is the axis whose middle
