@@ -244,6 +244,18 @@ int sn_bn_finalize(double* stats, int n, int c, int groups, int hw, float eps, f
                    float* running_var, long long* num_batches_tracked, void* stream);
 int sn_bn_eval_stats(double* stats, int n, int c, const float* running_mean, const float* running_var, float eps,
                      void* stream);
+/* Cross-rank batch statistics (data parallelism): every rank normalises with the statistics of each group's samples on
+ * all ranks.  sn_bn_group_sums turns per-(n, c) pair sums — the forward's (sum, sum of squares) or the backward's
+ * (sum g, sum g*xhat), see sn_norm_act_bwd_desc.bn_phase — into this rank's partials part[groups][c][3] =
+ * (element count n/groups * hw, sum, sum of squares), summing the samples in sample order.  The caller gathers every
+ * rank's part in rank order into gathered[world][groups][c][3] (the element count travels with the sums: shards may
+ * differ in size).  sn_bn_finalize_gathered sums those slices in rank order, writes the (mean, rstd) of each local
+ * sample's group to stats[n][c] and updates the running buffers as sn_bn_finalize does, with the unbiased variance over
+ * the global count: every rank computes the same bits.  With world 1 both give sn_bn_finalize's results exactly. */
+int sn_bn_group_sums(const double* stats, int n, int c, int groups, int hw, double* part, void* stream);
+int sn_bn_finalize_gathered(double* stats, int n, int c, int groups, const double* gathered, int world, float eps,
+                            float momentum, float* running_mean, float* running_var, long long* num_batches_tracked,
+                            void* stream);
 
 typedef struct sn_norm_act_desc {
   const float* y; int y_pitch;           /* conv output, [n, h, w, c] */
@@ -301,6 +313,13 @@ typedef struct sn_norm_act_bwd_desc {
   float* gamma_grad; float* beta_grad;   /* optional [c]: += d(loss)/d(gamma), d(loss)/d(beta) */
   double* det_slots; long long det_slots_cap; /* non-NULL: deterministic gstats reduction (see sn_det_slots; no
                                             fused bias_grad) */
+  int bn_phase;                          /* BatchNorm, train mode, statistics across ranks: the call is split so that the
+                                            gather of the gradient sums sits between its halves.  0: the whole backward
+                                            (all fields below zero).  1: the reduction only; gstats is left holding the
+                                            per-(n, c) (sum g, sum g*xhat) for sn_bn_group_sums.  2: group means from
+                                            bn_gathered, then the apply pass */
+  const double* bn_gathered; int bn_world; int bn_rank; /* phase 2: [bn_world][bn_groups][c][3] gathered partials,
+                                            this rank's index: d(gamma), d(beta) add its slice only */
 } sn_norm_act_bwd_desc;
 int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream);
 

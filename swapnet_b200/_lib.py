@@ -111,6 +111,7 @@ class SnNormActBwdDesc(C.Structure):
         ("gamma", C.c_void_p), ("beta", C.c_void_p), ("bn_groups", C.c_int), ("bn_train", C.c_int),
         ("gamma_grad", C.c_void_p), ("beta_grad", C.c_void_p),
         ("det_slots", C.c_void_p), ("det_slots_cap", C.c_longlong),
+        ("bn_phase", C.c_int), ("bn_gathered", C.c_void_p), ("bn_world", C.c_int), ("bn_rank", C.c_int),
     ]
 
 
@@ -143,6 +144,8 @@ SIGNATURES = {
     "sn_plane_sums": (_I, [_VP, _I, _I, _I, _I, _VP, _VP]),
     "sn_bn_finalize": (_I, [_VP, _I, _I, _I, _I, _F, _F, _VP, _VP, _VP, _VP]),
     "sn_bn_eval_stats": (_I, [_VP, _I, _I, _VP, _VP, _F, _VP]),
+    "sn_bn_group_sums": (_I, [_VP, _I, _I, _I, _I, _VP, _VP]),
+    "sn_bn_finalize_gathered": (_I, [_VP, _I, _I, _I, _VP, _I, _F, _F, _VP, _VP, _VP, _VP]),
     "sn_pack_planes": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_pack_concat": (_I, [_VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "sn_pack_head_weights": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _VP, _VP]),

@@ -508,6 +508,18 @@ __global__ void gstats_finalize_kernel(double* g, int count, int hw) {
 // (the discriminator's fake and real halves).  One thread per channel sums the samples in index order: no atomics,
 // the same result on every run.
 // ---------------------------------------------------------------------------------
+// One group's statistics from its element count and sums, shared by the single-process and the cross-rank kernels so
+// that the two cannot drift: (mean, 1/sqrt(var_biased + eps)) for the normalisation, and the running-buffer update
+__device__ __forceinline__ void bn_group_stat(double s1, double s2, double cnt, double eps, float momentum,
+                                              double& mean, double& rstd, float& rm, float& rv) {
+  mean = s1 / cnt;
+  double var = s2 / cnt - mean * mean;
+  if (var < 0) var = 0;
+  rstd = rsqrt(var + eps);
+  // torch: running <- (1 - momentum) * running + momentum * stat, the variance stat unbiased (n / (n - 1))
+  rm = (float)((1.0 - momentum) * rm + momentum * mean);
+  rv = (float)((1.0 - momentum) * rv + momentum * (cnt > 1 ? var * cnt / (cnt - 1) : var));
+}
 // stats[n][c] = (sum y, sum y^2) -> (mean_G, rstd_G) of the sample's group; running buffers updated group by group
 __global__ void bn_finalize_kernel(double* stats, int N, int C, int groups, int hw, double eps, float momentum,
                                    float* run_mean, float* run_var, long long* num_batches) {
@@ -523,17 +535,66 @@ __global__ void bn_finalize_kernel(double* stats, int N, int C, int groups, int 
       s1 += stats[((long long)n * C + c) * 2];
       s2 += stats[((long long)n * C + c) * 2 + 1];
     }
-    const double mean = s1 / cnt;
-    double var = s2 / cnt - mean * mean;
-    if (var < 0) var = 0;
-    const double rstd = rsqrt(var + eps);
+    double mean, rstd;
+    bn_group_stat(s1, s2, cnt, eps, momentum, mean, rstd, rm, rv);
     for (int n = gi * per; n < (gi + 1) * per; ++n) {
       stats[((long long)n * C + c) * 2] = mean;
       stats[((long long)n * C + c) * 2 + 1] = rstd;
     }
-    // torch: running <- (1 - momentum) * running + momentum * stat, the variance stat unbiased (n / (n - 1))
-    rm = (float)((1.0 - momentum) * rm + momentum * mean);
-    rv = (float)((1.0 - momentum) * rv + momentum * (cnt > 1 ? var * cnt / (cnt - 1) : var));
+  }
+  if (run_mean) run_mean[c] = rm;
+  if (run_var) run_var[c] = rv;
+}
+// Cross-rank batch statistics.  A rank's partials are part[g][c] = (element count, sum, sum of squares) of its samples
+// of group g; the ranks' slices are gathered in rank order into [world][groups][C][3] and summed in that order, so
+// every rank gets the same bits whatever the transport.  With one rank the sums are those of the kernels above.
+// part[g][c] = (per * hw, sum over the group's samples in sample order of stats[n][c]): the forward's (sum y, sum y^2)
+// or the backward's (sum g, sum g*xhat)
+__global__ void bn_group_sums_kernel(const double* stats, int N, int C, int groups, int hw, double* part) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int per = N / groups;
+  for (int gi = 0; gi < groups; ++gi) {
+    double s1 = 0.0, s2 = 0.0;
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      s1 += stats[((long long)n * C + c) * 2];
+      s2 += stats[((long long)n * C + c) * 2 + 1];
+    }
+    double* p = part + ((long long)gi * C + c) * 3;
+    p[0] = (double)per * hw;
+    p[1] = s1;
+    p[2] = s2;
+  }
+}
+// sum of the gathered slices of group gi, channel c, in rank order
+__device__ __forceinline__ void bn_gathered_sums(const double* gathered, int world, int groups, int C, int gi, int c,
+                                                 double& cnt, double& s1, double& s2) {
+  cnt = 0.0, s1 = 0.0, s2 = 0.0;
+  for (int r = 0; r < world; ++r) {
+    const double* p = gathered + (((long long)r * groups + gi) * C + c) * 3;
+    cnt += p[0];
+    s1 += p[1];
+    s2 += p[2];
+  }
+}
+// stats[n][c] <- (mean, rstd) of the sample's group over all ranks; running buffers updated group by group from the
+// global statistics (the same bits on every rank)
+__global__ void bn_finalize_gathered_kernel(double* stats, int N, int C, int groups, const double* gathered, int world,
+                                            double eps, float momentum, float* run_mean, float* run_var,
+                                            long long* num_batches) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c == 0 && num_batches) *num_batches += groups;
+  if (c >= C) return;
+  const int per = N / groups;
+  float rm = run_mean ? run_mean[c] : 0.f, rv = run_var ? run_var[c] : 0.f;
+  for (int gi = 0; gi < groups; ++gi) {
+    double cnt, s1, s2, mean, rstd;
+    bn_gathered_sums(gathered, world, groups, C, gi, c, cnt, s1, s2);
+    bn_group_stat(s1, s2, cnt, eps, momentum, mean, rstd, rm, rv);
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      stats[((long long)n * C + c) * 2] = mean;
+      stats[((long long)n * C + c) * 2 + 1] = rstd;
+    }
   }
   if (run_mean) run_mean[c] = rm;
   if (run_var) run_var[c] = rv;
@@ -568,6 +629,28 @@ __global__ void bn_bwd_group_kernel(double* g, int N, int C, int groups, int hw,
     for (int n = gi * per; n < (gi + 1) * per; ++n) {
       g[((long long)n * C + c) * 2] = train ? s1 / cnt : 0.0;
       g[((long long)n * C + c) * 2 + 1] = train ? s2 / cnt : 0.0;
+    }
+  }
+  if (dbeta) dbeta[c] += (float)tb;
+  if (dgamma) dgamma[c] += (float)tg;
+}
+// train mode across ranks: g[n][c] <- the global group means of (g, g*xhat) for the apply pass.  d(gamma), d(beta) add
+// this rank's sums only (its slice of `gathered`): the gradient all-reduce that follows sums them over the ranks
+__global__ void bn_bwd_group_gathered_kernel(double* g, int N, int C, int groups, const double* gathered, int world,
+                                             int rank, float* dgamma, float* dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int per = N / groups;
+  double tb = 0.0, tg = 0.0;
+  for (int gi = 0; gi < groups; ++gi) {
+    double cnt, s1, s2;
+    bn_gathered_sums(gathered, world, groups, C, gi, c, cnt, s1, s2);
+    const double* mine = gathered + (((long long)rank * groups + gi) * C + c) * 3;
+    tb += mine[1];
+    tg += mine[2];
+    for (int n = gi * per; n < (gi + 1) * per; ++n) {
+      g[((long long)n * C + c) * 2] = s1 / cnt;
+      g[((long long)n * C + c) * 2 + 1] = s2 / cnt;
     }
   }
   if (dbeta) dbeta[c] += (float)tb;
@@ -1826,6 +1909,27 @@ int sn_bn_finalize(double* stats, int n, int c, int groups, int hw, float eps, f
   return SN_OK;
 }
 
+int sn_bn_group_sums(const double* stats, int n, int c, int groups, int hw, double* part, void* stream) {
+  SN_REQUIRE(stats && part && n >= 1 && c >= 1 && hw >= 1, "bn_group_sums: bad arguments");
+  SN_REQUIRE(groups >= 1 && n % groups == 0, "bn_group_sums: %d samples do not split into %d groups", n, groups);
+  bn_group_sums_kernel<<<(c + 127) / 128, 128, 0, (cudaStream_t)stream>>>(stats, n, c, groups, hw, part);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_bn_finalize_gathered(double* stats, int n, int c, int groups, const double* gathered, int world, float eps,
+                            float momentum, float* running_mean, float* running_var, long long* num_batches_tracked,
+                            void* stream) {
+  SN_REQUIRE(stats && gathered && n >= 1 && c >= 1 && world >= 1, "bn_finalize_gathered: bad arguments");
+  SN_REQUIRE(groups >= 1 && n % groups == 0, "bn_finalize_gathered: %d samples do not split into %d groups", n, groups);
+  SN_REQUIRE((running_mean == nullptr) == (running_var == nullptr),
+             "bn_finalize_gathered: running mean and variance go together");
+  bn_finalize_gathered_kernel<<<(c + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      stats, n, c, groups, gathered, world, (double)eps, momentum, running_mean, running_var, num_batches_tracked);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
 int sn_bn_eval_stats(double* stats, int n, int c, const float* running_mean, const float* running_var, float eps,
                      void* stream) {
   SN_REQUIRE(stats && running_mean && running_var && n >= 1 && c >= 1, "bn_eval_stats: bad arguments");
@@ -1930,7 +2034,15 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
                    (d->dy_pitch % 4 == 0) && (d->dy_coff % 4 == 0) && ((uintptr_t)d->dy_hi & 7) == 0 &&
                    ((uintptr_t)d->dy_lo & 7) == 0 && d->c <= 2048;
   SN_REQUIRE(!aff || vec, "norm_act_bwd: the BatchNorm variant needs c %% 4 == 0 and 16-byte aligned rows (c=%d)", d->c);
-  if (d->stats) {
+  SN_REQUIRE(d->bn_phase >= 0 && d->bn_phase <= 2, "norm_act_bwd: bn_phase %d", d->bn_phase);
+  SN_REQUIRE(d->bn_phase == 0 || (aff && d->bn_train), "norm_act_bwd: bn_phase needs the BatchNorm variant in train mode");
+  SN_REQUIRE(d->bn_phase != 2 || (d->gstats && d->bn_gathered && d->bn_world >= 1 && d->bn_rank >= 0 && d->bn_rank < d->bn_world),
+             "norm_act_bwd: bn_phase 2 needs bn_gathered and 0 <= bn_rank < bn_world (%d, %d)", d->bn_rank, d->bn_world);
+  if (d->bn_phase == 2) {
+    bn_bwd_group_gathered_kernel<<<(d->c + 127) / 128, 128, 0, st>>>(d->gstats, d->n, d->c, d->bn_groups, d->bn_gathered,
+                                                                     d->bn_world, d->bn_rank, d->gamma_grad, d->beta_grad);
+    LAUNCH_CHECK();
+  } else if (d->stats) {
     SN_REQUIRE(d->gstats, "InstanceNorm backward needs gstats scratch");
     SN_CHECK_CUDA(cudaMemsetAsync(d->gstats, 0, sizeof(double) * 2 * d->n * d->c, st));
     int nslabs = 1;
@@ -1963,6 +2075,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       SN_CHECK_CUDA(det_sum_slots(d->det_slots, nslabs, 2LL * d->n * d->c, d->gstats, st));
       LAUNCH_CHECK();
     }
+    if (d->bn_phase == 1) return SN_OK;
     if (aff)
       bn_bwd_group_kernel<<<(d->c + 127) / 128, 128, 0, st>>>(d->gstats, d->n, d->c, d->bn_groups, hw, d->bn_train,
                                                               d->gamma_grad, d->beta_grad);

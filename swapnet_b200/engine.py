@@ -78,6 +78,10 @@ class Stage:
         self.dy: Optional[Planes] = None
         self.dx: Optional[torch.Tensor] = None
         self.gstats = None
+        # batch statistics across ranks: this rank's per-group partials and every rank's, gathered
+        self.bn_part = self.bn_gathered = None
+        if bn is not None and eng.bn_sync is not None:
+            self.bn_part, self.bn_gathered = eng.bn_sync.buffers(groups, self.cout, dev)
 
     def drop_offset(self) -> int:
         """Keep-mask index of this stage's first element: the masks are indexed by GLOBAL sample (Engine.sample_base =
@@ -110,7 +114,12 @@ class Stage:
             else:
                 if not fused:
                     ops.plane_sums(self.y, self.cout, self.stats, ws=self.eng.det_ws)
-                ops.bn_finalize(self.stats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn)
+                if self.bn_part is not None:
+                    ops.bn_group_sums(self.stats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn_part)
+                    self.eng.bn_sync.gather(self.bn_part, self.bn_gathered)
+                    ops.bn_finalize_gathered(self.stats, self.n, self.cout, self.groups, self.bn_gathered, self.bn)
+                else:
+                    ops.bn_finalize(self.stats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn)
         elif self.norm:
             if fused:
                 ops.stats_finalize(self.stats, self.n * self.cout, self.oh * self.ow)
@@ -162,11 +171,18 @@ class Stage:
                 bn = self._affine()
                 if wgrad and self.bn.weight.grad is not None:
                     bn_grads = (self.bn.weight.grad, self.bn.bias.grad)
-            ops.norm_act_bwd(srcs, self.y, self.cout, None if self.plain else self.stats,
-                             ACT_NONE if self.plain else self.act, self.dy, self.gstats, self.slope, p,
-                             _mix_seed(self.eng.seed, self.id), drop_offset=self.drop_offset(),
-                             seed_dev=self.eng.seed_dev, stage_id=self.id, bias_grad=bg, bn=bn, bn_groups=self.groups,
-                             bn_train=self.eng.training, bn_grads=bn_grads, ws=self.eng.det_ws)
+            args = (srcs, self.y, self.cout, None if self.plain else self.stats, ACT_NONE if self.plain else self.act,
+                    self.dy, self.gstats, self.slope, p, _mix_seed(self.eng.seed, self.id))
+            kw = dict(drop_offset=self.drop_offset(), seed_dev=self.eng.seed_dev, stage_id=self.id, bias_grad=bg, bn=bn,
+                      bn_groups=self.groups, bn_train=self.eng.training, bn_grads=bn_grads, ws=self.eng.det_ws)
+            if bn is not None and self.bn_part is not None and self.eng.training:
+                # the group means of (g, g*xhat) are global: reduce, gather the partials, then group and apply
+                ops.norm_act_bwd(*args, **kw, bn_phase=1)
+                ops.bn_group_sums(self.gstats, self.n, self.cout, self.groups, self.oh * self.ow, self.bn_part)
+                self.eng.bn_sync.gather(self.bn_part, self.bn_gathered)
+                ops.norm_act_bwd(*args, **kw, bn_phase=2, bn_gathered=self.bn_gathered, bn_rank=self.eng.bn_sync.rank)
+            else:
+                ops.norm_act_bwd(*args, **kw)
             if bg is not None:
                 self._layer_backward(wgrad, bias=False)
                 return
@@ -192,11 +208,15 @@ class Stage:
 class Engine:
     """Common plumbing: stage list, flat gradient buffer, packing."""
 
-    def __init__(self, net: nn.Module, device, nsplit: int, train: bool = True, deterministic: bool = False):
+    def __init__(self, net: nn.Module, device, nsplit: int, train: bool = True, deterministic: bool = False,
+                 bn_sync=None):
         """deterministic: every reduction that spans blocks adds its partial sums in a fixed order instead of with
-        floating-point atomics, so a step gives bit-identical results on every run (DESIGN.md §4)."""
+        floating-point atomics, so a step gives bit-identical results on every run (DESIGN.md §4).
+        bn_sync (parallel.BNStatsExchange): train-mode batch norm normalises with the statistics of every rank's
+        samples (DESIGN.md §7); None: with this process's samples."""
         self.net, self.device, self.nsplit = net, torch.device(device), nsplit
         self.deterministic = bool(deterministic)
+        self.bn_sync = bn_sync
         # slot workspaces of the deterministic reductions: one for the launching stream, one for the weight-gradient
         # stream (the two overlap)
         self.det_ws = ops.DetWorkspace(device) if deterministic else None
@@ -451,8 +471,8 @@ class PatchGANEngine(Engine):
 
     def __init__(self, net: M.NLayerDiscriminator, batch: int, size: int, device, nsplit: int = 3,
                  din: Optional[Planes] = None, input_grad: bool = False, train: bool = True, groups: int = 1,
-                 deterministic: bool = False):
-        super().__init__(net, device, nsplit, train, deterministic)
+                 deterministic: bool = False, bn_sync=None):
+        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
         B, S, dev = batch, size, self.device
         self.batch, self.size = B, S
         self.din = din if din is not None else self.planes(B, S, S, L.padc(net.input_nc))
@@ -509,8 +529,8 @@ class TextureEngine(Engine):
     """
 
     def __init__(self, net: M.TextureModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
-                 deterministic: bool = False):
-        super().__init__(net, device, nsplit, train, deterministic)
+                 deterministic: bool = False, bn_sync=None):
+        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
         B, S = batch, size
         assert S >= 64 and (S & (S - 1)) == 0, "texture stage: power-of-two size >= 64"
         self.batch, self.size = B, S

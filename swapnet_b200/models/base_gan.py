@@ -19,8 +19,10 @@ What runs differently from the eager reference (results unchanged):
   * losses stay on the device until get_current_losses() is called.
 Unsupported option values raise (there is no eager fallback): --gan_mode wgan-gp / dragan-gp / dragan-lp (the
 gradient penalty needs a second derivative through D), --gan_mode mescheder-r1-gp / mescheder-r2-gp (the reference's
-GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel, --norm batch
-under data parallelism (no cross-rank batch statistics).
+GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel.
+--norm batch under data parallelism needs --b200_sync_bn 1: every train-mode BatchNorm2d call then normalises with the
+statistics of all ranks' samples (parallel.BNStatsExchange), so that 2 ranks x B/2 samples still reproduce one process
+with the full batch B; without the flag it is refused, since per-rank statistics would quietly break that equivalence.
 """
 from __future__ import annotations
 
@@ -79,6 +81,18 @@ def deterministic_mode(opt) -> bool:
     return torch.are_deterministic_algorithms_enabled() if v is None else bool(v)
 
 
+def batch_norm_exchange(opt, world: int) -> Optional[parallel.BNStatsExchange]:
+    """The cross-rank statistics exchange of `--norm batch` under data parallelism with --b200_sync_bn 1; None where
+    batch statistics stay local (one rank, or no batch norm).  Without the flag the combination is refused: per-rank
+    statistics would quietly break the equivalence of 2 ranks x B/2 samples with one process and B samples."""
+    if opt.norm != "batch" or world <= 1:
+        return None
+    if not getattr(opt, "b200_sync_bn", 0):
+        raise NotImplementedError("--norm batch under data parallelism needs cross-rank batch statistics: pass "
+                                  "--b200_sync_bn 1, train on one GPU or use --norm instance / none")
+    return parallel.BNStatsExchange()
+
+
 class BaseGAN(BaseModel, ABC):
     @staticmethod
     def modify_commandline_options(parser: ArgumentParser, is_train):
@@ -115,6 +129,10 @@ class BaseGAN(BaseModel, ABC):
                             help="1: bit-identical steps on every run (reductions add their partial sums in a fixed "
                                  "order instead of with floating-point atomics); 0: the default kernels.  Default: "
                                  "torch.are_deterministic_algorithms_enabled() when the model is built")
+        parser.add_argument("--b200_sync_bn", type=int, default=0, choices=(0, 1),
+                            help="1: under data parallelism, --norm batch normalises with the batch statistics of "
+                                 "every rank's samples (exchanged each call, summed in rank order); no effect on one "
+                                 "GPU.  0: --norm batch with more than one rank is refused")
         parser.add_argument("--b200_precision", default="fp32x3", choices=("fp32x3", "bf16"),
                             help="tensor-core arithmetic of the B200 engines: fp32x3 = split-bf16 3-pass "
                                  "(fp32-faithful, parity mode); bf16 = single pass (fast, ~1e-2 relative)")
@@ -138,6 +156,7 @@ class BaseGAN(BaseModel, ABC):
         # smooth-label draws: the CPU default generator like the reference (loss.py:74-77); under DP a
         # dedicated, identically seeded generator so that every rank sees the same label (SURVEY §8e i)
         self._labels = parallel.LabelDraws(1234 if self._world > 1 else None)
+        self._bn_sync: Optional[parallel.BNStatsExchange] = None   # cross-rank batch statistics (--b200_sync_bn 1)
         if self.is_train:
             if opt.gan_mode in ("wgan-gp", "dragan-gp", "dragan-lp"):
                 raise NotImplementedError(f"--gan_mode {opt.gan_mode}: its gradient penalty needs a second derivative "
@@ -151,9 +170,7 @@ class BaseGAN(BaseModel, ABC):
                                           "not provided")
             if opt.discriminator == "pixel":
                 raise NotImplementedError("--discriminator pixel is not provided on the B200 engines")
-            if opt.norm == "batch" and self._world > 1:
-                raise NotImplementedError("--norm batch under data parallelism: cross-rank batch statistics (SyncBN) "
-                                          "are not implemented; train on one GPU or use --norm instance / none")
+            self._bn_sync = batch_norm_exchange(opt, self._world)
             n_layers = 3 if opt.discriminator == "basic" else opt.n_layers_D
             self.net_discriminator = M.NLayerDiscriminator(self.get_D_inchannels(), 64, n_layers, opt.norm).to(self.device)
             M.init_weights(self.net_discriminator, opt.init_type, opt.init_gain)
@@ -253,12 +270,12 @@ class BaseGAN(BaseModel, ABC):
             # the D step's fake and real halves are two D calls: with batch norm, two sample groups with their own
             # statistics and running-buffer updates (fake first)
             dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit, groups=2,
-                                            deterministic=self.deterministic)
+                                            deterministic=self.deterministic, bn_sync=self._bn_sync)
             dd.alloc_grads()
             dd.bind_backward()
             dg = e["Dg"] = E.PatchGANEngine(dn, batch, size, self.device, self.nsplit,
                                             din=dd.din.batch_slice(0, batch), input_grad=True,
-                                            deterministic=self.deterministic)
+                                            deterministic=self.deterministic, bn_sync=self._bn_sync)
             dg.alloc_grads(share_with=dd)
             dg.bind_backward(wgrad=False)
             e["dpred_d"] = torch.zeros_like(dd.pred)

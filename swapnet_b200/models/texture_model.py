@@ -88,7 +88,7 @@ class TextureModel(BaseGAN):
 
     def build_generator_engine(self, batch, size):
         return E.TextureEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train,
-                               deterministic=self.deterministic)
+                               deterministic=self.deterministic, bn_sync=self._bn_sync)
 
     def _build_engines(self, batch, size):
         e = super()._build_engines(batch, size)

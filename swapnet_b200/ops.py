@@ -587,6 +587,29 @@ def bn_finalize(stats: torch.Tensor, n: int, c: int, groups: int, hw: int, bn: "
                                      _ptr(bn.num_batches_tracked if track else None), _stream()))
 
 
+def bn_group_sums(stats: torch.Tensor, n: int, c: int, groups: int, hw: int, part: torch.Tensor) -> None:
+    """Per-(n, c) pair sums (the forward's (sum, sum of squares) or, after norm_act_bwd(bn_phase=1), the backward's
+    (sum g, sum g*xhat)) -> this rank's partials part [groups, c, 3] fp64 = (element count, sum, sum of squares)."""
+    assert stats.dtype == part.dtype == torch.float64 and n % groups == 0 and part.numel() >= groups * c * 3
+    check(_lib.load().sn_bn_group_sums(stats.data_ptr(), n, c, groups, hw, part.data_ptr(), _stream()))
+
+
+def bn_finalize_gathered(stats: torch.Tensor, n: int, c: int, groups: int, gathered: torch.Tensor,
+                         bn: "torch.nn.BatchNorm2d") -> None:
+    """bn_finalize with the statistics of every rank: gathered [world, groups, c, 3] fp64 holds the ranks'
+    bn_group_sums partials in rank order; stats [n, c, 2] <- (mean, rstd) of each local sample's global group, and bn's
+    running buffers are updated from the global statistics."""
+    assert stats.dtype == gathered.dtype == torch.float64 and n % groups == 0
+    assert gathered.dim() == 4 and tuple(gathered.shape[1:]) == (groups, c, 3) and gathered.is_contiguous()
+    assert bn.momentum is not None, "BatchNorm2d(momentum=None) (cumulative average) is not provided"
+    track = bn.track_running_stats
+    check(_lib.load().sn_bn_finalize_gathered(stats.data_ptr(), n, c, groups, gathered.data_ptr(), gathered.shape[0],
+                                              float(bn.eps), float(bn.momentum),
+                                              _ptr(bn.running_mean if track else None),
+                                              _ptr(bn.running_var if track else None),
+                                              _ptr(bn.num_batches_tracked if track else None), _stream()))
+
+
 def bn_eval_stats(stats: torch.Tensor, n: int, c: int, bn: "torch.nn.BatchNorm2d") -> None:
     """Eval-mode BatchNorm2d: stats [n, c, 2] <- (running_mean, rstd of running_var)."""
     assert stats.dtype == torch.float64
@@ -660,12 +683,16 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
                  stage_id: int = 0, bias_grad: Optional[torch.Tensor] = None,
                  bn: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, bn_groups: int = 1, bn_train: bool = True,
                  bn_grads: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
-                 ws: Optional[DetWorkspace] = None) -> None:
+                 ws: Optional[DetWorkspace] = None, bn_phase: int = 0, bn_gathered: Optional[torch.Tensor] = None,
+                 bn_rank: int = 0) -> None:
     """ws: deterministic reduction of the normalisation's gradient statistics (then no fused bias_grad).
     bias_grad (fp32 [c], c in {256, 512, 1024}): += per-channel sums of the dy written — the bias gradient of the
     conv that produced y — inside the apply pass (see fused_bias_grad_ok).
     bn = (gamma, beta): BatchNorm backward over `bn_groups` sample groups, with batch (bn_train) or running statistics
-    in `stats`; bn_grads = (d gamma, d beta) are accumulated (+=) when given."""
+    in `stats`; bn_grads = (d gamma, d beta) are accumulated (+=) when given.
+    Batch statistics across ranks split the call in two around the gather: bn_phase=1 leaves the per-(n, c)
+    (sum g, sum g*xhat) in gstats (for bn_group_sums); bn_phase=2 takes the group means from bn_gathered
+    [world, bn_groups, c, 3] and runs the apply pass, adding only rank bn_rank's sums to bn_grads."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)
     d = SnNormActBwdDesc()
@@ -690,6 +717,11 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
     if ws is not None and stats is not None:
         sl = ws.slots(n, c)
         d.det_slots, d.det_slots_cap = sl.data_ptr(), sl.numel()
+    d.bn_phase = bn_phase
+    if bn_gathered is not None:
+        assert bn_gathered.dtype == torch.float64 and bn_gathered.is_contiguous()
+        assert bn_gathered.dim() == 4 and tuple(bn_gathered.shape[1:]) == (bn_groups, c, 3)
+        d.bn_gathered, d.bn_world, d.bn_rank = bn_gathered.data_ptr(), bn_gathered.shape[0], bn_rank
     check(_lib.load().sn_norm_act_bwd(C.byref(d), _stream()))
 
 

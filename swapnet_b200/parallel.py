@@ -4,7 +4,8 @@ The hot path shards over the batch with no data-path collective: convs, Instance
 ROIAlign and the batch-mean losses are all per-sample, so equal shards + gradient averaging
 reproduce the single-process gradient (SURVEY §8e).  The only exchange step is one all-reduce of
 the flat fp32 gradient buffer per optimizer step; the smooth-label scalars (one draw per loss call
-for the whole batch, loss.py:65-77) come from an identically seeded generator on every rank.
+for the whole batch, loss.py:65-77) come from an identically seeded generator on every rank.  Batch norm couples the
+samples of a call: with `--b200_sync_bn 1` its statistics are exchanged per call (BNStatsExchange).
 """
 from __future__ import annotations
 
@@ -84,6 +85,36 @@ class BucketedAverager:
             self.work.clear()
             if self.scale:
                 self.flat.mul_(1.0 / w)
+
+
+class BNStatsExchange:
+    """Cross-rank batch-norm statistics (`--b200_sync_bn 1`): each BatchNorm2d call of a training step contributes its
+    per-group partials ([groups, C, 3] fp64: element count, sum, sum of squares; ops.bn_group_sums) and receives every
+    rank's, stacked in rank order ([world, groups, C, 3]).  The kernels sum the slices in that order, so every rank
+    computes the same bits whatever the transport's reduction algorithm, and unequal shards are weighted by their counts.
+
+    The exchange has a process group of its own: the gradient all-reduces that overlap the backward pass
+    (BucketedAverager) queue on the default group's communicator, and a gather behind a large bucket there would stall
+    the backward chain.  Every rank issues the gathers in the same order (the launch sequence is fixed), so they need no
+    further synchronisation.  `group`: an existing process group (tests pass a gloo group)."""
+
+    def __init__(self, group=None):
+        self.group = group if group is not None else dist.new_group()
+        self.world = dist.get_world_size(self.group)
+        self.rank = dist.get_rank(self.group)
+        self.gathers = 0            # gathers issued so far (the cost of the exchange is one latency-bound gather each)
+
+    def buffers(self, groups: int, c: int, device) -> tuple:
+        """(part [groups, c, 3], gathered [world, groups, c, 3]): fp64 buffers of one BatchNorm2d call site."""
+        part = torch.zeros(groups, c, 3, dtype=torch.float64, device=device)
+        return part, torch.zeros(self.world, groups, c, 3, dtype=torch.float64, device=device)
+
+    def gather(self, part: torch.Tensor, gathered: torch.Tensor) -> torch.Tensor:
+        """gathered[r] <- rank r's part, on the current stream."""
+        assert part.is_contiguous() and gathered.is_contiguous() and gathered.numel() == self.world * part.numel()
+        dist.all_gather_into_tensor(gathered.view(-1), part.view(-1), group=self.group)
+        self.gathers += 1
+        return gathered
 
 
 def broadcast_parameters(params: Iterable[torch.Tensor], src: int = 0) -> None:
