@@ -486,6 +486,44 @@ int sn_gram(const float* src, long long s_n, long long s_c, long long s_p, int n
 int sn_gram_det(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
                 double* gram, double* slots, long long slots_cap, void* stream);
 long long sn_gram_det_slots(int rows);
+
+/* ------------------------------------------------------------------------------------------
+ * 1x1 PixelGAN discriminator (discriminators.py:138-168, csrc/pixel_disc.cu): per pixel
+ *   z1 = W1 x + b1 (64), a1 = lrelu(z1), z2 = W2 a1 (+ b2) (128), y2 = InstanceNorm(z2) or z2, a2 = lrelu(y2),
+ *   pred = w3 . a2 (+ b3).
+ * Every pass recomputes z1 and z2 from x through one device function (bit-identical in every pass); nothing of the
+ * hidden layers is stored.  Weights are the torch parameters themselves ([64][cin], [128][64], [1][128]).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct sn_pixel_desc {
+  const void* x_hi; const void* x_lo;     /* fp16-split operand planes [n*hw][x_pitch] (forward products) */
+  const void* xb_hi; const void* xb_lo;   /* their bf16-split twin (dW1 in sn_pixel_bwd_apply) */
+  int x_pitch, x_c;                        /* x_c = 16 or 32 channels read, zero from cin on */
+  int n, hw, cin;
+  const float* w1; const float* b1; const float* w2; const float* b2; const float* w3; const float* b3;  /* b2, b3 may be
+                                            NULL (--norm none: no bias on net.2 / net.5) */
+  const float* scale1; const float* scale2;  /* device (s, 1/s) of w1 and w2 from sn_weight_scale_multi */
+  int norm;                                /* 1: InstanceNorm2d(affine=False) after net.2, 0: none */
+  int nsplit;                              /* 3 = split products, 1 = hi x hi only */
+  float slope, eps;                        /* LeakyReLU slope (0.2), InstanceNorm eps */
+  double* stats;                           /* [n][128][2]: (mean, rstd) of z2 per (image, channel) */
+  double* gstats;                          /* [n][128][2]: (sum g2, sum g2 * y2) */
+  float* pred;                             /* [n*hw] logits */
+  const float* dpred;                      /* [n*hw] dL/dpred */
+  float* dw1; float* db1; float* dw2; float* db2; float* dw3; float* db3;   /* += gradients; NULL: not computed */
+  float* dx; int dx_pitch;                 /* optional fp32 NHWC [n*hw][dx_pitch]: dL/dx, channels < cin */
+  float* debug;                            /* optional [n*hw][64 + 128]: z1 and y2 (sn_pixel_fwd) */
+  double* slots; long long slots_cap;      /* non-NULL: deterministic reductions (sn_pixel_det_slots doubles) */
+} sn_pixel_desc;
+/* stats <- (mean, rstd): per-(n, c) sum z2 and sum z2^2 in fp64, then sn_stats_finalize (norm = 1 only) */
+int sn_pixel_fwd_stats(const sn_pixel_desc* d, void* stream);
+/* pred (and debug) */
+int sn_pixel_fwd(const sn_pixel_desc* d, void* stream);
+/* gstats <- (sum g2, sum g2 * y2), g2 = dpred w3 lrelu'(y2); dw3 += sum dpred a2, db3 += sum dpred (norm = 1 only) */
+int sn_pixel_bwd_reduce(const sn_pixel_desc* d, void* stream);
+/* dz2 (the InstanceNorm backward, or g2), dw2/db2, g1 = (W2^T dz2) lrelu'(z1), dw1/db1, dx = W1^T g1; with norm = 0 also
+ * dw3/db3 */
+int sn_pixel_bwd_apply(const sn_pixel_desc* d, void* stream);
+long long sn_pixel_det_slots(int n, int cin);
 /* *loss_acc += weight * MSELoss(gram_out, gram_tgt);  m[r][j] = d(that)/d(gram_out) + transpose (fp32). */
 int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double weight, double* loss_acc, float* m,
                 void* stream);

@@ -115,6 +115,20 @@ class SnNormActBwdDesc(C.Structure):
     ]
 
 
+class SnPixelDesc(C.Structure):
+    _fields_ = [
+        ("x_hi", C.c_void_p), ("x_lo", C.c_void_p), ("xb_hi", C.c_void_p), ("xb_lo", C.c_void_p),
+        ("x_pitch", C.c_int), ("x_c", C.c_int), ("n", C.c_int), ("hw", C.c_int), ("cin", C.c_int),
+        ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p), ("w3", C.c_void_p),
+        ("b3", C.c_void_p), ("scale1", C.c_void_p), ("scale2", C.c_void_p),
+        ("norm", C.c_int), ("nsplit", C.c_int), ("slope", C.c_float), ("eps", C.c_float),
+        ("stats", C.c_void_p), ("gstats", C.c_void_p), ("pred", C.c_void_p), ("dpred", C.c_void_p),
+        ("dw1", C.c_void_p), ("db1", C.c_void_p), ("dw2", C.c_void_p), ("db2", C.c_void_p), ("dw3", C.c_void_p),
+        ("db3", C.c_void_p), ("dx", C.c_void_p), ("dx_pitch", C.c_int), ("debug", C.c_void_p),
+        ("slots", C.c_void_p), ("slots_cap", C.c_longlong),
+    ]
+
+
 # name -> (restype, argtypes); every symbol declared in include/swapnet_b200.h
 _VP, _I, _LL, _F, _ULL = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_ulonglong
 SIGNATURES = {
@@ -193,6 +207,11 @@ SIGNATURES = {
     "sn_gram_bwd": (_I, [_VP, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _I, _I, _VP]),
     "sn_roi_align_pack_fwd": (_I, [_VP, _I, _I, _I, _I, _VP, _I, _I, _VP, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_tap_gemm_simt": (_I, [C.POINTER(SnTapGemmDesc), _VP]),
+    "sn_pixel_fwd_stats": (_I, [C.POINTER(SnPixelDesc), _VP]),
+    "sn_pixel_fwd": (_I, [C.POINTER(SnPixelDesc), _VP]),
+    "sn_pixel_bwd_reduce": (_I, [C.POINTER(SnPixelDesc), _VP]),
+    "sn_pixel_bwd_apply": (_I, [C.POINTER(SnPixelDesc), _VP]),
+    "sn_pixel_det_slots": (_LL, [_I, _I]),
     "sn_augment_channels": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _I, _I, _VP, _VP, _VP]),
 }
 

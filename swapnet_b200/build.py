@@ -16,7 +16,8 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libswapnet_b200.so")
-SOURCES = ["api.cu", "gemm_tc.cu", "elementwise.cu", "roi_align.cu", "perceptual.cu", "patch_logits.cu", "augment.cu"]
+SOURCES = ["api.cu", "gemm_tc.cu", "elementwise.cu", "roi_align.cu", "perceptual.cu", "patch_logits.cu", "augment.cu",
+           "pixel_disc.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

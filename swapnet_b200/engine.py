@@ -513,6 +513,70 @@ class PatchGANEngine(Engine):
         return self.chain[0].dx
 
 
+class PixelGANEngine(Engine):
+    """PixelDiscriminator (the 1x1 PatchGAN) on a [batch, S, S, padc(input_nc)] operand (`self.din`), with the surface
+    of PatchGANEngine.  Its hidden layers run at full resolution and are never stored: the four passes of
+    csrc/pixel_disc.cu recompute them from `din`, so the engine holds only the logits `pred` [batch, S, S], the
+    per-(image, channel) statistics and, with input_grad, `dx_in`."""
+
+    def __init__(self, net: M.PixelDiscriminator, batch: int, size: int, device, nsplit: int = 3,
+                 din: Optional[Planes] = None, input_grad: bool = False, train: bool = True, groups: int = 1,
+                 deterministic: bool = False, bn_sync=None):
+        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
+        if net.norm == "batch":
+            raise NotImplementedError("--discriminator pixel --norm batch: batch statistics couple the samples inside "
+                                      "the fused per-pixel passes, which normalise per image; use --norm instance or "
+                                      "none")
+        B, S, dev = batch, size, self.device
+        self.batch, self.size = B, S
+        self.din = din if din is not None else self.planes(B, S, S, L.padc(net.input_nc))
+        assert (self.din.n, self.din.h, self.din.w) == (B, S, S) and self.din.c in (16, 32)
+        self.pred = torch.zeros(B, S, S, device=dev)
+        norm = net.norm == "instance"
+        self.stats = torch.zeros(B, 128, 2, dtype=torch.float64, device=dev) if norm else None
+        self.gstats = torch.zeros_like(self.stats) if norm else None
+        self.scales = torch.zeros(2, 2, device=dev)          # (s, 1/s) of net.0 and net.2 weights
+        cin = net.input_nc
+        self.dx = torch.zeros(B, S, S, (cin + 3) // 4 * 4, device=dev)[..., :cin] if input_grad else None
+        self.debug: Optional[torch.Tensor] = None             # [B*S*S, 64 + 128]: z1 and y2 of the forward (tests)
+
+    def workspace_bytes(self) -> int:
+        return 0 if self.det_ws is None else self.det_ws.nbytes
+
+    def pack(self) -> None:
+        """The power-of-two scales of the (updated) net.0 and net.2 weights; the passes split the weights themselves."""
+        if self._pack_table is None:
+            self._pack_table = ops.PackTable(self.device)
+            self._pack_table.add_scale(self.net.net[0].weight.data, self.scales[0])
+            self._pack_table.add_scale(self.net.net[2].weight.data, self.scales[1])
+        self._pack_table.run()
+
+    def _desc(self, **kw):
+        return ops.pixel_desc(self.din, self.net, self.scales, self.nsplit, stats=self.stats, gstats=self.gstats, **kw)
+
+    def forward(self) -> torch.Tensor:
+        if self.stats is not None:
+            ops.pixel_pass("fwd_stats", self._desc(), ws=self.det_ws)
+        ops.pixel_pass("fwd", self._desc(pred=self.pred, debug=self.debug))
+        return self.pred
+
+    def backward(self, dpred: torch.Tensor, wgrad: bool = True) -> None:
+        grads = {}
+        if wgrad:
+            c0, c2, c5 = self.net.net[0], self.net.net[2], self.net.net[5]
+            grads = dict(dw1=c0.weight.grad, db1=c0.bias.grad, dw2=c2.weight.grad,
+                         db2=None if c2.bias is None else c2.bias.grad, dw3=c5.weight.grad,
+                         db3=None if c5.bias is None else c5.bias.grad)
+        if self.stats is not None:
+            ops.pixel_pass("bwd_reduce", self._desc(dpred=dpred, **grads), ws=self.det_ws)
+        dx = dict(dx=self.dx, dx_pitch=self.dx.stride(2)) if self.dx is not None else {}
+        ops.pixel_pass("bwd_apply", self._desc(dpred=dpred, **grads, **dx), ws=self.det_ws)
+
+    @property
+    def dx_in(self) -> torch.Tensor:
+        return self.dx
+
+
 # =============================================================================================
 # TextureModule
 # =============================================================================================

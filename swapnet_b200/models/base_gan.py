@@ -3,7 +3,8 @@
 Keeps the option surface and step order of /root/reference/models/base_gan.py:16-231:
     forward -> zero/backward/step D -> zero/backward/step G        (base_gan.py:194-203)
 with G = a generator engine, D = the conditional PatchGAN (define_D 'basic' / 'n_layers',
-discriminators.py:45-88), GANLoss (loss.py:12-130) for --gan_mode vanilla (BCE-with-logits), lsgan (MSE) and wgan
+discriminators.py:45-88) or the 1x1 PixelGAN ('pixel', discriminators.py:138-168; engine.PixelGANEngine), GANLoss
+(loss.py:12-130) for --gan_mode vanilla (BCE-with-logits), lsgan (MSE) and wgan
 (-mean(pred) for real, +mean(pred) for fake) and torch.optim.AdamW or adabound.AdaBound (--optimizer_G / --optimizer_D,
 chosen per network) exactly as optimizers/__init__.py:37-60 builds them.
 vanilla and lsgan use the reference's smooth labels (loss.py:65-108, including the "fake target drawn from the real
@@ -19,7 +20,8 @@ What runs differently from the eager reference (results unchanged):
   * losses stay on the device until get_current_losses() is called.
 Unsupported option values raise (there is no eager fallback): --gan_mode wgan-gp / dragan-gp / dragan-lp (the
 gradient penalty needs a second derivative through D), --gan_mode mescheder-r1-gp / mescheder-r2-gp (the reference's
-GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel.
+GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel with
+--norm batch (batch statistics would couple the samples inside its fused per-pixel passes).
 --norm batch under data parallelism needs --b200_sync_bn 1: every train-mode BatchNorm2d call then normalises with the
 statistics of all ranks' samples (parallel.BNStatsExchange), so that 2 ranks x B/2 samples still reproduce one process
 with the full batch B; without the flag it is refused, since per-rank statistics would quietly break that equivalence.
@@ -168,11 +170,17 @@ class BaseGAN(BaseModel, ABC):
             if opt.gan_label_mode != "smooth":
                 raise NotImplementedError("--gan_label_mode hard crashes in the reference (loss.py:92,101) and is "
                                           "not provided")
-            if opt.discriminator == "pixel":
-                raise NotImplementedError("--discriminator pixel is not provided on the B200 engines")
+            if opt.discriminator == "pixel" and opt.norm == "batch":
+                raise NotImplementedError("--discriminator pixel --norm batch is not provided: batch statistics couple "
+                                          "the samples inside the fused per-pixel passes (csrc/pixel_disc.cu), which "
+                                          "normalise per image; use --norm instance or none")
             self._bn_sync = batch_norm_exchange(opt, self._world)
-            n_layers = 3 if opt.discriminator == "basic" else opt.n_layers_D
-            self.net_discriminator = M.NLayerDiscriminator(self.get_D_inchannels(), 64, n_layers, opt.norm).to(self.device)
+            if opt.discriminator == "pixel":     # --n_layers_D is ignored, as in the reference
+                self.net_discriminator = M.PixelDiscriminator(self.get_D_inchannels(), 64, opt.norm).to(self.device)
+            else:
+                n_layers = 3 if opt.discriminator == "basic" else opt.n_layers_D
+                self.net_discriminator = M.NLayerDiscriminator(self.get_D_inchannels(), 64, n_layers,
+                                                               opt.norm).to(self.device)
             M.init_weights(self.net_discriminator, opt.init_type, opt.init_gain)
             self.model_names.append("discriminator")
             if opt.lambda_discriminator:
@@ -269,13 +277,13 @@ class BaseGAN(BaseModel, ABC):
             dn = self.net_discriminator
             # the D step's fake and real halves are two D calls: with batch norm, two sample groups with their own
             # statistics and running-buffer updates (fake first)
-            dd = e["Dd"] = E.PatchGANEngine(dn, 2 * batch, size, self.device, self.nsplit, groups=2,
-                                            deterministic=self.deterministic, bn_sync=self._bn_sync)
+            D = E.PixelGANEngine if isinstance(dn, M.PixelDiscriminator) else E.PatchGANEngine
+            dd = e["Dd"] = D(dn, 2 * batch, size, self.device, self.nsplit, groups=2,
+                             deterministic=self.deterministic, bn_sync=self._bn_sync)
             dd.alloc_grads()
             dd.bind_backward()
-            dg = e["Dg"] = E.PatchGANEngine(dn, batch, size, self.device, self.nsplit,
-                                            din=dd.din.batch_slice(0, batch), input_grad=True,
-                                            deterministic=self.deterministic, bn_sync=self._bn_sync)
+            dg = e["Dg"] = D(dn, batch, size, self.device, self.nsplit, din=dd.din.batch_slice(0, batch), input_grad=True,
+                             deterministic=self.deterministic, bn_sync=self._bn_sync)
             dg.alloc_grads(share_with=dd)
             dg.bind_backward(wgrad=False)
             e["dpred_d"] = torch.zeros_like(dd.pred)

@@ -4,6 +4,7 @@ These nn.Modules hold ONLY the trainable tensors, under exactly the state_dict k
 construction / nn.Module.apply order, so that a seeded init matches) of the reference networks:
   WarpModule           /root/reference/modules/swapnet_modules.py:22-90
   NLayerDiscriminator  /root/reference/modules/discriminators.py:91-132
+  PixelDiscriminator   /root/reference/modules/discriminators.py:138-168
   TextureModule        /root/reference/modules/swapnet_modules.py:154-207
   UnetGenerator        /root/reference/modules/pix2pix_modules.py:113-262
 Checkpoints are therefore interchangeable with the reference (`base_model.py:156-213`).  The
@@ -125,6 +126,20 @@ class NLayerDiscriminator(_NoEager):
         """The BatchNorm2d after each conv (None where there is none), aligned with convs()."""
         return [self.model[i + 1] if isinstance(self.model[i + 1], nn.BatchNorm2d) else None
                 for i in self.conv_index[:-1]] + [None]
+
+
+class PixelDiscriminator(_NoEager):
+    """The 1x1 PatchGAN ('pixel', discriminators.py:138-168): net.0 Conv 1x1 input_nc -> ndf (bias), net.1 LeakyReLU,
+    net.2 Conv ndf -> 2 ndf, net.3 the norm slot, net.4 LeakyReLU, net.5 Conv 2 ndf -> 1.  As in the reference, net.2 and
+    net.5 have a bias only with InstanceNorm2d.  ndf = 64 only (csrc/pixel_disc.cu's widths)."""
+
+    def __init__(self, input_nc, ndf=64, norm="instance"):
+        super().__init__()
+        self.norm, self.input_nc, self.ndf = check_norm(norm), input_nc, ndf
+        use_bias = norm == "instance"    # discriminators.py:150-153
+        self.net = nn.Sequential(nn.Conv2d(input_nc, ndf, 1), nn.Identity(),
+                                 nn.Conv2d(ndf, ndf * 2, 1, bias=use_bias), _norm_slot(norm, ndf * 2), nn.Identity(),
+                                 nn.Conv2d(ndf * 2, 1, 1, bias=use_bias))
 
 
 class _SkipBlock(_NoEager):

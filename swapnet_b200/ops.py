@@ -1087,3 +1087,36 @@ def to_one_dgrad(dy: Planes, weight: torch.Tensor, pad: int, dx: torch.Tensor) -
     assert (dy.h, dy.w) == (h + 2 * pad - 3, w + 2 * pad - 3)
     check(_lib.load().sn_to_one_dgrad(dy.hi_ptr, dy.lo_ptr, dy.pitch, dy.fmt, n, h, w, weight.shape[1],
                                       weight.data_ptr(), 4, pad, dx.data_ptr(), _pitch(dx), _stream()))
+
+
+# ---------------------------------------------------------------------------------------------
+# 1x1 PixelGAN discriminator (csrc/pixel_disc.cu)
+# ---------------------------------------------------------------------------------------------
+def pixel_desc(x: Planes, net, scales: torch.Tensor, nsplit: int, **kw) -> "_lib.SnPixelDesc":
+    """Descriptor of the PixelGAN passes over the operand planes x [n, h, w, 16 | 32] (fp16-split; its bf16 twin feeds
+    dW1).  net: modules.PixelDiscriminator; scales [2, 2]: (s, 1/s) of net.0 and net.2 weights (weight_scale_multi).
+    kw: the remaining sn_pixel_desc fields, tensors or None."""
+    d = _lib.SnPixelDesc()
+    d.x_hi, d.x_lo = x.hi_ptr, x.lo_ptr
+    if x.twin is not None:
+        d.xb_hi, d.xb_lo = x.twin.hi_ptr, x.twin.lo_ptr
+    d.x_pitch, d.x_c, d.n, d.hw, d.cin = x.pitch, x.c, x.n, x.h * x.w, net.input_nc
+    c0, c2, c5 = net.net[0], net.net[2], net.net[5]
+    d.w1, d.b1, d.w2, d.b2 = c0.weight.data_ptr(), c0.bias.data_ptr(), c2.weight.data_ptr(), _ptr(c2.bias)
+    d.w3, d.b3 = c5.weight.data_ptr(), _ptr(c5.bias)
+    d.scale1, d.scale2 = scales[0].data_ptr(), scales[1].data_ptr()
+    d.norm, d.nsplit, d.slope, d.eps = int(net.norm == "instance"), nsplit, 0.2, IN_EPS
+    for k, v in kw.items():
+        setattr(d, k, v.data_ptr() if torch.is_tensor(v) else v)
+    return d
+
+
+def pixel_pass(name: str, d: "_lib.SnPixelDesc", ws: Optional[DetWorkspace] = None) -> None:
+    """One PixelGAN pass: name in fwd_stats, fwd, bwd_reduce, bwd_apply.  ws: deterministic reductions."""
+    lib = _lib.load()
+    if ws is not None:
+        sl = ws.get(int(lib.sn_pixel_det_slots(d.n, d.cin)))
+        d.slots, d.slots_cap = sl.data_ptr(), sl.numel()
+    else:
+        d.slots, d.slots_cap = None, 0
+    check(getattr(lib, "sn_pixel_" + name)(C.byref(d), _stream()))
