@@ -9,9 +9,9 @@ import sys as _sys
 
 from swapnet_b200 import models as _impl
 from swapnet_b200.models import BaseModel, create_model  # noqa: F401
-from swapnet_b200.models import base_gan, base_model, texture_model, warp_model  # noqa: F401
+from swapnet_b200.models import base_gan, base_model, pix2pix_model, texture_model, warp_model  # noqa: F401
 
-for _name in ("base_model", "base_gan", "warp_model", "texture_model"):
+for _name in ("base_model", "base_gan", "warp_model", "texture_model", "pix2pix_model"):
     _sys.modules[f"{__name__}.{_name}"] = getattr(_impl, _name)
 
 

@@ -164,12 +164,13 @@ int sn_wgrad_ksplit(const sn_wgrad_desc* desc, int sm_count);
 int sn_pack_planes(const float* src, int src_layout, int src_pitch, int n, int c, int h, int w,
                    void* dst_hi, void* dst_lo, int dst_pitch, int dst_coff, int fmt, void* stream);
 
-/* one pass: up to two fp32 sources (src1 may be NULL) concatenated along channels and zero-filled to
- * c_fill channels -> planes (dst_*) and, optionally, a second-format copy (dst2_*, e.g. the bf16 twin).
- * dst_coff, c_fill, dst_pitch multiples of 8.  (cat((bodys, fakes), 1) of warp_model.py:115 etc.) */
-int sn_pack_concat(const float* src0, int layout0, int pitch0, int c0, const float* src1, int layout1, int pitch1,
-                   int c1, int n, int h, int w, int c_fill, void* dst_hi, void* dst_lo, void* dst2_hi, void* dst2_lo,
-                   int dst_pitch, int dst_coff, int fmt, int fmt2, void* stream);
+/* one pass: `lead` zero channels, then up to two fp32 sources (src1 may be NULL) concatenated along channels and
+ * zero-filled to c_fill channels -> planes (dst_*) and, optionally, a second-format copy (dst2_*, e.g. the bf16 twin).
+ * dst_coff, c_fill, dst_pitch multiples of 8; lead any count >= 0 (pix2pix's cat(zeros[B, 36], cloths),
+ * pix2pix_model.py:158-159).  (cat((bodys, fakes), 1) of warp_model.py:115 etc.) */
+int sn_pack_concat(int lead, const float* src0, int layout0, int pitch0, int c0, const float* src1, int layout1,
+                   int pitch1, int c1, int n, int h, int w, int c_fill, void* dst_hi, void* dst_lo, void* dst2_hi,
+                   void* dst2_lo, int dst_pitch, int dst_coff, int fmt, int fmt2, void* stream);
 
 /* weight packing: torch conv weights -> kernel-layout split planes, a whole network in one launch per entry.  The item
  * tables live in DEVICE memory and are built once per engine.

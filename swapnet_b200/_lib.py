@@ -161,7 +161,7 @@ SIGNATURES = {
     "sn_bn_group_sums": (_I, [_VP, _I, _I, _I, _I, _VP, _VP]),
     "sn_bn_finalize_gathered": (_I, [_VP, _I, _I, _I, _VP, _I, _F, _F, _VP, _VP, _VP, _VP]),
     "sn_pack_planes": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
-    "sn_pack_concat": (_I, [_VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "sn_pack_concat": (_I, [_I, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "sn_pack_head_weights": (_I, [_VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _VP, _VP]),
     "sn_weight_scale_multi": (_I, [_VP, _I, _VP, _VP]),
     "sn_pack_weights_multi": (_I, [_VP, _I, _I, _I, _VP]),

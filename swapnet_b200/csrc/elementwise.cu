@@ -112,14 +112,15 @@ __global__ void pack_planes_nhwc_kernel(const float* __restrict__ src, int src_p
   }
 }
 
-// pack_concat: up to two fp32 sources (NCHW or NHWC) concatenated along channels, zero-filled up to
-// c_fill channels, written as full 16-byte groups of 8 channels into the fp16 planes AND their bf16
-// twin in one pass.  One block = one (n, h, 32-pixel run).
+// pack_concat: `lead` zero channels, then up to two fp32 sources (NCHW or NHWC) concatenated along channels,
+// zero-filled up to c_fill channels, written as full 16-byte groups of 8 channels into the fp16 planes AND their
+// bf16 twin in one pass.  One block = one (n, h, 32-pixel run).
 struct PackSrc { const float* p; int layout, pitch, c; };
 struct PackConcatArgs {
   PackSrc s[2]; int nsrc;
   int N, H, W, c_fill;
   uint16_t *hi, *lo, *hi2, *lo2; int pitch, coff, fmt, fmt2;
+  int lead;                 // zero channels in front of the sources
 };
 __global__ void __launch_bounds__(256) pack_concat_kernel(const PackConcatArgs a) {
   // one block = one (n, h, PW-pixel run), PW = 32 * (64 / c_fill) so that narrow outputs keep all
@@ -128,7 +129,7 @@ __global__ void __launch_bounds__(256) pack_concat_kernel(const PackConcatArgs a
   const int PW = 32 * (64 / (a.c_fill < 64 ? a.c_fill : 64));
   const int TP = PW + 1;
   const int w0 = blockIdx.x * PW, h = blockIdx.y, n = blockIdx.z;
-  int cbase = 0;
+  int cbase = a.lead;
   for (int si = 0; si < a.nsrc; ++si) {
     const PackSrc s = a.s[si];
     if (s.layout == SN_LAYOUT_NCHW) {
@@ -149,7 +150,11 @@ __global__ void __launch_bounds__(256) pack_concat_kernel(const PackConcatArgs a
     }
     cbase += s.c;
   }
-  for (int i = threadIdx.x; i < (a.c_fill - cbase) * PW; i += blockDim.x) tile[(cbase + i / PW) * TP + (i % PW)] = 0.f;
+  // zero channels: the lead [0, lead) and the fill [cbase, c_fill)
+  for (int i = threadIdx.x; i < (a.lead + a.c_fill - cbase) * PW; i += blockDim.x) {
+    const int z = i / PW;
+    tile[(z < a.lead ? z : cbase + z - a.lead) * TP + (i % PW)] = 0.f;
+  }
   __syncthreads();
   const int G = a.c_fill >> 3;
   for (int i = threadIdx.x; i < PW * G; i += blockDim.x) {
@@ -192,7 +197,7 @@ __global__ void __launch_bounds__(256) pack_concat_direct_kernel(const PackConca
     float v[CF];
 #pragma unroll
     for (int c = 0; c < CF; ++c) v[c] = 0.f;
-    int cbase = 0;
+    int cbase = a.lead;
     for (int si = 0; si < a.nsrc; ++si) {
       const PackSrc s = a.s[si];
       if (s.layout == SN_LAYOUT_NCHW) {
@@ -1762,11 +1767,12 @@ int sn_pack_planes(const float* src, int src_layout, int src_pitch, int n, int c
   return SN_OK;
 }
 
-int sn_pack_concat(const float* src0, int layout0, int pitch0, int c0, const float* src1, int layout1, int pitch1,
-                   int c1, int n, int h, int w, int c_fill, void* dst_hi, void* dst_lo, void* dst2_hi, void* dst2_lo,
-                   int dst_pitch, int dst_coff, int fmt, int fmt2, void* stream) {
+int sn_pack_concat(int lead, const float* src0, int layout0, int pitch0, int c0, const float* src1, int layout1,
+                   int pitch1, int c1, int n, int h, int w, int c_fill, void* dst_hi, void* dst_lo, void* dst2_hi,
+                   void* dst2_lo, int dst_pitch, int dst_coff, int fmt, int fmt2, void* stream) {
   SN_REQUIRE(src0 && dst_hi, "null pointer");
-  SN_REQUIRE(c_fill % 8 == 0 && dst_coff % 8 == 0 && dst_pitch % 8 == 0 && c0 + (src1 ? c1 : 0) <= c_fill &&
+  SN_REQUIRE(lead >= 0, "pack_concat: negative zero lead (%d)", lead);
+  SN_REQUIRE(c_fill % 8 == 0 && dst_coff % 8 == 0 && dst_pitch % 8 == 0 && lead + c0 + (src1 ? c1 : 0) <= c_fill &&
                  dst_coff + c_fill <= dst_pitch,
              "pack_concat: channel slice must be 8-aligned and fit (coff=%d fill=%d pitch=%d)", dst_coff, c_fill,
              dst_pitch);
@@ -1776,6 +1782,7 @@ int sn_pack_concat(const float* src0, int layout0, int pitch0, int c0, const flo
   a.s[0] = PackSrc{src0, layout0, pitch0, c0};
   a.s[1] = PackSrc{src1, layout1, pitch1, src1 ? c1 : 0};
   a.nsrc = src1 ? 2 : 1;
+  a.lead = lead;
   a.N = n; a.H = h; a.W = w; a.c_fill = c_fill;
   a.hi = (uint16_t*)dst_hi; a.lo = (uint16_t*)dst_lo; a.hi2 = (uint16_t*)dst2_hi; a.lo2 = (uint16_t*)dst2_lo;
   a.pitch = dst_pitch; a.coff = dst_coff; a.fmt = fmt; a.fmt2 = fmt2;

@@ -578,56 +578,41 @@ class PixelGANEngine(Engine):
 
 
 # =============================================================================================
-# TextureModule
+# pix2pix U-Net (shared by TextureModule and the standalone generator)
 # =============================================================================================
-class TextureEngine(Engine):
-    """ROIAlign+repack -> encode (UNetDown 36->36) -> nearest upsample -> cat cloth -> pix2pix U-Net
-    (swapnet_modules.py:231-260, pix2pix_modules.py:113-262; the U-Net's [IN] below is its norm: instance (bias on
-    every conv), batch (BatchNorm2d, no bias but on U_0) or none (no bias but on U_0); `encode` is always IN).
+class UNetStages:
+    """The stages of an M.UnetGenerator on an engine, reading the operand planes `x` and writing `fakes` (fp32 NHWC,
+    tanh) — pix2pix_modules.py:113-262; the norm is the container's: instance (bias on every conv), batch (BatchNorm2d,
+    no bias but on U_0) or none (no bias but on U_0).
 
-    U-Net bookkeeping (depth j = 0 outermost .. nd-1 innermost; D_j / U_j = its down / up conv):
+    Bookkeeping (depth j = 0 outermost .. nd-1 innermost; D_j / U_j = its down / up conv):
       L_{j+1} = leaky_relu([IN](D_j(.)))  is both the operand of D_{j+1} and, because the reference's
                 LeakyReLU is in place, the skip half of block j+1's output (App. B #1);
       the parent applies ReLU to the whole concat, so U_j reads cat(relu(L_{j+1}), relu(V_{j+1})) with
       V = dropout?(IN(U(.))) — buffer `cu[j]`, written in place by the producing stages.
-    """
+    Stages are created on `eng` in the order D_0..D_{nd-1}, U_{nd-1}..U_0 (their ids seed the dropout masks)."""
 
-    def __init__(self, net: M.TextureModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
-                 deterministic: bool = False, bn_sync=None):
-        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
-        B, S = batch, size
-        assert S >= 64 and (S & (S - 1)) == 0, "texture stage: power-of-two size >= 64"
-        self.batch, self.size = B, S
-        self.ct, self.cc, self.nroi = net.texture_channels, net.cloth_channels, net.num_roi
-        ch = self.ct * self.nroi
-        self.ch = ch
-        unet = net.unet
+    def __init__(self, eng: Engine, unet: M.UnetGenerator, x: Planes, fakes: torch.Tensor, input_grad: bool = True):
+        """input_grad: D_0 computes the gradient w.r.t. `x` (`dx`)."""
+        B, S = x.n, x.h
         nd = unet.num_downs
         blocks = unet.blocks()
         assert len(blocks) == nd
-        self.pool = 128
-        self.pooled = self.planes(B, self.pool, self.pool, L.padc(ch))
-        self.enc = self.planes(B, self.pool // 2, self.pool // 2, L.padc(ch))
-        self.in_unet = self.planes(B, S, S, L.padc(ch + self.cc))
-        self.up_factor = S // (self.pool // 2)
-        St = lambda *a, **k: Stage(self, *a, **k)  # noqa: E731
-        self.encode = St("encode", "conv4s2", net.encode.model[0], self.pooled, out=self.enc, norm=True,
-                         act=ACT_LRELU, need_dx=False)
+        St = lambda *a, **k: Stage(eng, *a, **k)  # noqa: E731
         chans = [blocks[j].down.out_channels for j in range(nd)]          # channels of x_{j+1}
-        self.cu = [self.planes(B, S >> (j + 1), S >> (j + 1), 2 * chans[j]) for j in range(nd - 1)]
+        self.cu = [eng.planes(B, S >> (j + 1), S >> (j + 1), 2 * chans[j]) for j in range(nd - 1)]
         use_norm = unet.norm != "none"
         self.down: List[Stage] = []
-        x = self.in_unet
         for j in range(nd):
             h = S >> (j + 1)
             last = j == nd - 1
+            out = eng.planes(B, h, h, L.padc(chans[j]))
             if last:
-                out = self.planes(B, h, h, L.padc(chans[j]))
                 st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=False, act=ACT_RELU)
             else:
-                out = self.planes(B, h, h, L.padc(chans[j]))
-                st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=(j >= 1) and use_norm, act=ACT_LRELU,
-                        out_relu=self.cu[j].slice(0, chans[j]), bn=blocks[j].down_bn)
+                st = St(f"unet.D{j}", "conv4s2", blocks[j].down, x, out=out, norm=(j >= 1) and use_norm,
+                        act=ACT_LRELU, out_relu=self.cu[j].slice(0, chans[j]), bn=blocks[j].down_bn,
+                        need_dx=(j > 0) or input_grad)
             self.down.append(st)
             x = out
         self.up: List[Optional[Stage]] = [None] * nd
@@ -637,28 +622,16 @@ class TextureEngine(Engine):
             drop = 0.5 if (blocks[j].use_dropout and not blocks[j].innermost) else 0.0
             self.up[j] = St(f"unet.U{j}", "convT4s2", blocks[j].up, src, out=self.cu[j - 1].slice(chans[j - 1], cout),
                             norm=use_norm, act=ACT_RELU, drop_p=drop, bn=blocks[j].up_bn)
-        self.fakes = torch.zeros(B, S, S, self.ct, device=self.device)
-        self.up[0] = St("unet.U0", "convT4s2", blocks[0].up, self.cu[0], plain=True, epi_act=ACT_TANH, y=self.fakes)
+        self.up[0] = St("unet.U0", "convT4s2", blocks[0].up, self.cu[0], plain=True, epi_act=ACT_TANH, y=fakes)
 
-    def forward(self, tex: torch.Tensor, rois: torch.Tensor, cloth: torch.Tensor, training: bool = True,
-                seed: int = 0, before_cloth=None) -> torch.Tensor:
-        """tex [B,3,S,S], rois [B,12,4], cloth [B,19,S,S] (fp32, device) -> fakes [B,S,S,3] NHWC."""
-        self.training, self.seed = training, seed
-        ops.roi_align_pack(tex, rois, self.pool, None, self.pooled.slice(0, self.ch))
-        if self.pooled.twin is not None:
-            ops.roi_align_pack(tex, rois, self.pool, None, self.pooled.twin.slice(0, self.ch))
-        self.encode.forward()
-        ops.upsample_planes(self.enc.slice(0, self.ch), self.in_unet.slice(0, self.ch), self.up_factor)
-        if before_cloth is not None:       # the plugin waits here for the cloth's H2D copy
-            before_cloth()
-        ops.pack_planes(cloth, self.in_unet.slice(self.ch, self.cc))
+    def forward(self) -> None:
         for st in self.down:
             st.forward()
         for j in range(len(self.up) - 1, -1, -1):
             self.up[j].forward()
-        return self.fakes
 
-    def backward(self, srcs: Sequence[GradSrc]) -> None:
+    def backward(self, srcs: Sequence[GradSrc]) -> Optional[torch.Tensor]:
+        """srcs: gradient(s) w.r.t. fakes.  Returns d/dx (D_0's `dx`; None without input_grad)."""
         nd = len(self.down)
         self.up[0].backward(srcs)
         g = self.up[0].dx                                           # d cu[0]
@@ -674,7 +647,85 @@ class TextureEngine(Engine):
         for j in range(nd - 2, -1, -1):
             # L_{j+1} feeds D_{j+1} (as leaky_relu) and the skip slot of cu[j] (as relu)
             self.down[j].backward([GradSrc(self.down[j + 1].dx), GradSrc(gcu[j], 0, act=ACT_RELU)])
-        self.encode.backward([GradSrc(self.down[0].dx, 0, up=self.up_factor)])
+        return self.down[0].dx
+
+
+# =============================================================================================
+# TextureModule
+# =============================================================================================
+class TextureEngine(Engine):
+    """ROIAlign+repack -> encode (UNetDown 36->36) -> nearest upsample -> cat cloth -> pix2pix U-Net
+    (swapnet_modules.py:231-260; the U-Net is UNetStages; `encode` is always IN)."""
+
+    def __init__(self, net: M.TextureModule, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
+                 deterministic: bool = False, bn_sync=None):
+        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
+        B, S = batch, size
+        assert S >= 64 and (S & (S - 1)) == 0, "texture stage: power-of-two size >= 64"
+        self.batch, self.size = B, S
+        self.ct, self.cc, self.nroi = net.texture_channels, net.cloth_channels, net.num_roi
+        ch = self.ct * self.nroi
+        self.ch = ch
+        self.pool = 128
+        self.pooled = self.planes(B, self.pool, self.pool, L.padc(ch))
+        self.enc = self.planes(B, self.pool // 2, self.pool // 2, L.padc(ch))
+        self.in_unet = self.planes(B, S, S, L.padc(ch + self.cc))
+        self.up_factor = S // (self.pool // 2)
+        self.encode = Stage(self, "encode", "conv4s2", net.encode.model[0], self.pooled, out=self.enc, norm=True,
+                            act=ACT_LRELU, need_dx=False)
+        self.fakes = torch.zeros(B, S, S, self.ct, device=self.device)
+        self.unet = UNetStages(self, net.unet, self.in_unet, self.fakes)
+
+    def forward(self, tex: torch.Tensor, rois: torch.Tensor, cloth: torch.Tensor, training: bool = True,
+                seed: int = 0, before_cloth=None) -> torch.Tensor:
+        """tex [B,3,S,S], rois [B,12,4], cloth [B,19,S,S] (fp32, device) -> fakes [B,S,S,3] NHWC."""
+        self.training, self.seed = training, seed
+        ops.roi_align_pack(tex, rois, self.pool, None, self.pooled.slice(0, self.ch))
+        if self.pooled.twin is not None:
+            ops.roi_align_pack(tex, rois, self.pool, None, self.pooled.twin.slice(0, self.ch))
+        self.encode.forward()
+        ops.upsample_planes(self.enc.slice(0, self.ch), self.in_unet.slice(0, self.ch), self.up_factor)
+        if before_cloth is not None:       # the plugin waits here for the cloth's H2D copy
+            before_cloth()
+        ops.pack_planes(cloth, self.in_unet.slice(self.ch, self.cc))
+        self.unet.forward()
+        return self.fakes
+
+    def backward(self, srcs: Sequence[GradSrc]) -> None:
+        dx = self.unet.backward(srcs)
+        self.encode.backward([GradSrc(dx, 0, up=self.up_factor)])
+        self.join_wgrads()
+
+
+class UnetEngine(Engine):
+    """A bare M.UnetGenerator (the pix2pix generator; `--netG unet_128` of the texture stage) on the operand planes
+    `x_in` [batch, S, S, padc(input_nc)], which the caller packs; output `fakes` [batch, S, S, output_nc] (fp32 NHWC,
+    tanh).  No input gradient.  S must be a multiple of 2**num_downs: the innermost level is then at least 1 x 1 (the
+    reference fails on mismatched skip concatenations otherwise)."""
+
+    def __init__(self, net: M.UnetGenerator, batch: int, size: int, device, nsplit: int = 3, train: bool = True,
+                 deterministic: bool = False, bn_sync=None):
+        super().__init__(net, device, nsplit, train, deterministic, bn_sync)
+        nd = net.num_downs
+        if size % (1 << nd) != 0:
+            raise ValueError(f"a U-Net with {nd} downsamplings needs an image size divisible by 2**{nd} = {1 << nd}, "
+                             f"got {size}: its skip connections would not line up")
+        B, S = batch, size
+        self.batch, self.size = B, S
+        blocks = net.blocks()
+        self.x_in = self.planes(B, S, S, L.padc(blocks[0].down.in_channels))
+        self.fakes = torch.zeros(B, S, S, blocks[0].up.out_channels, device=self.device)
+        self.unet = UNetStages(self, net, self.x_in, self.fakes, input_grad=False)
+
+    def forward(self, training: bool = True, seed: int = 0) -> torch.Tensor:
+        """x_in (packed by the caller) -> fakes [B,S,S,output_nc] NHWC."""
+        self.training, self.seed = training, seed
+        self.unet.forward()
+        return self.fakes
+
+    def backward(self, srcs: Sequence[GradSrc]) -> None:
+        """srcs: gradient(s) w.r.t. fakes; accumulates the parameter gradients into flat_grad."""
+        self.unet.backward(srcs)
         self.join_wgrads()
 
 

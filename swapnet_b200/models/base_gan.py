@@ -83,16 +83,42 @@ def deterministic_mode(opt) -> bool:
     return torch.are_deterministic_algorithms_enabled() if v is None else bool(v)
 
 
-def batch_norm_exchange(opt, world: int) -> Optional[parallel.BNStatsExchange]:
-    """The cross-rank statistics exchange of `--norm batch` under data parallelism with --b200_sync_bn 1; None where
+def batch_norm_exchange(opt, world: int, batch_norm: Optional[bool] = None) -> Optional[parallel.BNStatsExchange]:
+    """The cross-rank statistics exchange of batch norm under data parallelism with --b200_sync_bn 1; None where
     batch statistics stay local (one rank, or no batch norm).  Without the flag the combination is refused: per-rank
-    statistics would quietly break the equivalence of 2 ranks x B/2 samples with one process and B samples."""
-    if opt.norm != "batch" or world <= 1:
+    statistics would quietly break the equivalence of 2 ranks x B/2 samples with one process and B samples.
+    batch_norm: whether some network of the model has BatchNorm2d layers (default: `--norm batch`; a generator such as
+    `--netG unet_128` has them whatever --norm says)."""
+    if batch_norm is None:
+        batch_norm = opt.norm == "batch"
+    if not batch_norm or world <= 1:
         return None
     if not getattr(opt, "b200_sync_bn", 0):
+        if opt.norm != "batch":
+            raise NotImplementedError("the generator's batch norm under data parallelism needs cross-rank batch "
+                                      "statistics: pass --b200_sync_bn 1 or train on one GPU")
         raise NotImplementedError("--norm batch under data parallelism needs cross-rank batch statistics: pass "
                                   "--b200_sync_bn 1, train on one GPU or use --norm instance / none")
     return parallel.BNStatsExchange()
+
+
+def add_b200_options(parser: ArgumentParser) -> ArgumentParser:
+    """The engine switches every GAN plugin accepts, in training and at test time."""
+    parser.add_argument("--b200_graph", type=int, default=1, choices=(0, 1),
+                        help="1: replay the training step as a captured CUDA graph (single GPU; after two eager "
+                             "steps per input shape); 0: launch the kernels one by one")
+    parser.add_argument("--b200_deterministic", type=int, default=None, choices=(0, 1),
+                        help="1: bit-identical steps on every run (reductions add their partial sums in a fixed "
+                             "order instead of with floating-point atomics); 0: the default kernels.  Default: "
+                             "torch.are_deterministic_algorithms_enabled() when the model is built")
+    parser.add_argument("--b200_sync_bn", type=int, default=0, choices=(0, 1),
+                        help="1: under data parallelism, batch norm normalises with the batch statistics of "
+                             "every rank's samples (exchanged each call, summed in rank order); no effect on one "
+                             "GPU.  0: batch norm with more than one rank is refused")
+    parser.add_argument("--b200_precision", default="fp32x3", choices=("fp32x3", "bf16"),
+                        help="tensor-core arithmetic of the B200 engines: fp32x3 = split-bf16 3-pass "
+                             "(fp32-faithful, parity mode); bf16 = single pass (fast, ~1e-2 relative)")
+    return parser
 
 
 class BaseGAN(BaseModel, ABC):
@@ -124,21 +150,7 @@ class BaseGAN(BaseModel, ABC):
             parser.add_argument("--gan_label_mode", default="smooth", choices=("hard", "smooth"),
                                 help="whether to use hard (real 1.0 and fake 0.0) or smooth "
                                      "(real [0.7, 1.1] and fake [0., 0.3]) values for labels")
-        parser.add_argument("--b200_graph", type=int, default=1, choices=(0, 1),
-                            help="1: replay the training step as a captured CUDA graph (single GPU; after two eager "
-                                 "steps per input shape); 0: launch the kernels one by one")
-        parser.add_argument("--b200_deterministic", type=int, default=None, choices=(0, 1),
-                            help="1: bit-identical steps on every run (reductions add their partial sums in a fixed "
-                                 "order instead of with floating-point atomics); 0: the default kernels.  Default: "
-                                 "torch.are_deterministic_algorithms_enabled() when the model is built")
-        parser.add_argument("--b200_sync_bn", type=int, default=0, choices=(0, 1),
-                            help="1: under data parallelism, --norm batch normalises with the batch statistics of "
-                                 "every rank's samples (exchanged each call, summed in rank order); no effect on one "
-                                 "GPU.  0: --norm batch with more than one rank is refused")
-        parser.add_argument("--b200_precision", default="fp32x3", choices=("fp32x3", "bf16"),
-                            help="tensor-core arithmetic of the B200 engines: fp32x3 = split-bf16 3-pass "
-                                 "(fp32-faithful, parity mode); bf16 = single pass (fast, ~1e-2 relative)")
-        return parser
+        return add_b200_options(parser)
 
     def __init__(self, opt):
         super().__init__(opt)
@@ -160,13 +172,7 @@ class BaseGAN(BaseModel, ABC):
         self._labels = parallel.LabelDraws(1234 if self._world > 1 else None)
         self._bn_sync: Optional[parallel.BNStatsExchange] = None   # cross-rank batch statistics (--b200_sync_bn 1)
         if self.is_train:
-            if opt.gan_mode in ("wgan-gp", "dragan-gp", "dragan-lp"):
-                raise NotImplementedError(f"--gan_mode {opt.gan_mode}: its gradient penalty needs a second derivative "
-                                          "through D, which the engines do not compute (DESIGN.md §1)")
-            if opt.gan_mode not in ops.GAN_OBJECTIVES:
-                raise NotImplementedError(f"--gan_mode {opt.gan_mode}: the reference's GANLoss does not implement it "
-                                          "either (loss.py:61-62)")
-            self._gan_obj = ops.GAN_OBJECTIVES[opt.gan_mode]
+            self._gan_obj = self.gan_objective(opt.gan_mode)
             if opt.gan_label_mode != "smooth":
                 raise NotImplementedError("--gan_label_mode hard crashes in the reference (loss.py:92,101) and is "
                                           "not provided")
@@ -174,22 +180,22 @@ class BaseGAN(BaseModel, ABC):
                 raise NotImplementedError("--discriminator pixel --norm batch is not provided: batch statistics couple "
                                           "the samples inside the fused per-pixel passes (csrc/pixel_disc.cu), which "
                                           "normalise per image; use --norm instance or none")
-            self._bn_sync = batch_norm_exchange(opt, self._world)
+            self._bn_sync = batch_norm_exchange(opt, self._world, opt.norm == "batch" or any(
+                isinstance(m, torch.nn.BatchNorm2d) for m in self.net_generator.modules()))
             if opt.discriminator == "pixel":     # --n_layers_D is ignored, as in the reference
                 self.net_discriminator = M.PixelDiscriminator(self.get_D_inchannels(), 64, opt.norm).to(self.device)
             else:
                 n_layers = 3 if opt.discriminator == "basic" else opt.n_layers_D
                 self.net_discriminator = M.NLayerDiscriminator(self.get_D_inchannels(), 64, n_layers,
                                                                opt.norm).to(self.device)
-            M.init_weights(self.net_discriminator, opt.init_type, opt.init_gain)
+            self.init_D_weights(self.net_discriminator)
             self.model_names.append("discriminator")
-            if opt.lambda_discriminator:
+            if getattr(opt, "lambda_discriminator", 1.0):
                 self.loss_names = ["D", "D_real", "D_fake"]
             self.loss_names += ["G"]
             if opt.lambda_gan:
                 self.loss_names += ["G_gan"]
-            self.optimizer_G = define_optimizer(self.net_generator, opt, "G")
-            self.optimizer_D = define_optimizer(self.net_discriminator, opt, "D")
+            self.optimizer_G, self.optimizer_D = self.define_optimizers()
             self.optimizer_names = ("G", "D")
             self._acc = torch.zeros(8, dtype=torch.float64, device=self.device)  # device-side loss sums
             # per-step scalars read by the kernels from DEVICE memory (one tiny launch per step writes them), so that the
@@ -201,13 +207,35 @@ class BaseGAN(BaseModel, ABC):
             self._eager_steps = {}
             self.graph_enabled = bool(getattr(opt, "b200_graph", 1))
             self._acc_host = None                       # host copy of _acc for the current step (one D2H per step)
-            lam = float(opt.lambda_gan)
+            lam = self.gan_weight()
             self.loss_D_fake = LazyLoss(lambda: self.loss_values()[0])
             self.loss_D_real = LazyLoss(lambda: self.loss_values()[1])
             self.loss_D = LazyLoss(lambda: 0.5 * (self.loss_values()[0] + self.loss_values()[1]))
             self.loss_G_gan = LazyLoss(lambda: lam * self.loss_values()[2])
             parallel.broadcast_parameters(list(self.net_generator.parameters()) +
                                           list(self.net_discriminator.parameters()))
+
+    # ---- where a plugin departs from the reference's BaseGAN (pix2pix_model.py) ----
+    def gan_objective(self, mode: str) -> int:
+        """--gan_mode -> the ops.GAN_* objective the loss kernels run."""
+        if mode in ("wgan-gp", "dragan-gp", "dragan-lp"):
+            raise NotImplementedError(f"--gan_mode {mode}: its gradient penalty needs a second derivative "
+                                      "through D, which the engines do not compute (DESIGN.md §1)")
+        if mode not in ops.GAN_OBJECTIVES:
+            raise NotImplementedError(f"--gan_mode {mode}: the reference's GANLoss does not implement it "
+                                      "either (loss.py:61-62)")
+        return ops.GAN_OBJECTIVES[mode]
+
+    def gan_weight(self) -> float:
+        """Weight of the generator's GAN term."""
+        return float(self.opt.lambda_gan)
+
+    def init_D_weights(self, net) -> None:
+        M.init_weights(net, self.opt.init_type, self.opt.init_gain)
+
+    def define_optimizers(self):
+        """(optimizer_G, optimizer_D)."""
+        return define_optimizer(self.net_generator, self.opt, "G"), define_optimizer(self.net_discriminator, self.opt, "D")
 
     # ---- to be provided by the plugin ----
     @abstractmethod
@@ -357,7 +385,7 @@ class BaseGAN(BaseModel, ABC):
         g.pack()
         pred = g.forward()
         t = self._targets(2, 3, (-1.0,))
-        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 1, t, float(self.opt.lambda_gan), self._acc[2:3], self._dpred_g,
+        ops.gan_loss_fwd_bwd(self._gan_obj, pred, 1, t, self.gan_weight(), self._acc[2:3], self._dpred_g,
                              ws=self._det_ws)
         g.backward(self._dpred_g, wgrad=False)
         return g.dx_in

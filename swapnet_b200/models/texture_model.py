@@ -1,8 +1,10 @@
 """Texture-stage plugin (`--model texture`) on the B200 engines.
 
-Options, attributes and step semantics of /root/reference/models/texture_model.py:17-180 for the
-`--netG swapnet` generator (TextureModule): conditional PatchGAN on cat(cloths, texture) (cloth
-FIRST, :138,142,164), loss_G = lambda_gan * GAN + lambda_l1 * L1 (+ perceptual terms).
+Options, attributes and step semantics of /root/reference/models/texture_model.py:17-180 for both of its
+generators: `--netG swapnet` (TextureModule, on engine.TextureEngine) and `--netG unet_128` (a bare 7-level
+UnetGenerator with batch norm whatever --norm says and dropout, fed the input texture alone; the rois are unused:
+texture_model.py:96-101,121-125; on engine.UnetEngine).  Either way: conditional PatchGAN on cat(cloths, texture)
+(cloth FIRST, :138,142,164), loss_G = lambda_gan * GAN + lambda_l1 * L1 (+ perceptual terms).
 
 The VGG16 perceptual terms (texture_model.py:68-69,171-178 -> modules/losses/perceptual.py) run on
 engine.PerceptualEngine.  `vgg16(pretrained=True)` needs the torchvision weight file: `--b200_vgg`
@@ -38,8 +40,10 @@ class TextureModel(BaseGAN):
         return parser
 
     def __init__(self, opt):
-        if getattr(opt, "netG", "swapnet") != "swapnet":
-            raise NotImplementedError("--netG unet_128 (the reference's debugging generator) is not provided")
+        # at test time --netG is not an option: it comes from the saved training options (inference.py)
+        self.netG = getattr(opt, "netG", "swapnet")
+        if self.netG not in ("swapnet", "unet_128"):
+            raise ValueError("Cannot find implementation for " + self.netG)
         BaseGAN.__init__(self, opt)
         self.visual_names = ["textures_unnormalized", "cloths_decoded", "fakes", "fakes_scaled"]
         if self.is_train:
@@ -82,11 +86,17 @@ class TextureModel(BaseGAN):
         return self.opt.texture_channels + self.opt.cloth_channels
 
     def define_G(self):
+        if self.netG == "unet_128":
+            ct = self.opt.texture_channels
+            return M.UnetGenerator(ct, ct, 7, 64, use_dropout=True, norm="batch")
         return M.TextureModule(texture_channels=self.opt.texture_channels, cloth_channels=self.opt.cloth_channels,
                                num_roi=self.opt.body_channels, img_size=self.opt.crop_size,
                                norm_type=getattr(self.opt, "norm", "instance"))
 
     def build_generator_engine(self, batch, size):
+        if self.netG == "unet_128":
+            return E.UnetEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train,
+                                deterministic=self.deterministic, bn_sync=self._bn_sync)
         return E.TextureEngine(self.net_generator, batch, size, self.device, self.nsplit, train=self.is_train,
                                deterministic=self.deterministic, bn_sync=self._bn_sync)
 
@@ -119,9 +129,14 @@ class TextureModel(BaseGAN):
         g = self._eng_G
         g.pack()                      # needs the weights only: overlaps the input copies
         self.wait_copy("textures")
-        self.wait_copy("rois")
-        out = g.forward(self.textures, self.rois, self.cloths, training=self.training and self.is_train,
-                        seed=self.step_seed(), before_cloth=lambda: self.wait_copy("cloths"))
+        training = self.training and self.is_train
+        if self.netG == "unet_128":
+            ops.pack_concat([(self.textures, False)], g.x_in)
+            out = g.forward(training=training, seed=self.step_seed())
+        else:
+            self.wait_copy("rois")
+            out = g.forward(self.textures, self.rois, self.cloths, training=training, seed=self.step_seed(),
+                            before_cloth=lambda: self.wait_copy("cloths"))
         self.fakes = out.permute(0, 3, 1, 2)
         self.wait_late_copies()
 

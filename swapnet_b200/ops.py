@@ -419,11 +419,12 @@ def pack_planes(src, dst: Planes, *, nhwc: bool = False) -> None:
     assert (n, h, w) == (dst.n, dst.h, dst.w)
 
 
-def pack_concat(srcs, dst: Planes) -> None:
-    """srcs: 1-2 tuples (tensor, nhwc: bool); channels concatenated, zero-filled to dst.c, written to dst
-    and its twin in one pass.  Replaces cat((a, b), 1) + the channel padding of the operand."""
-    assert 1 <= len(srcs) <= 2 and dst.c % 8 == 0 and dst.c_off % 8 == 0
-    args = []
+def pack_concat(srcs, dst: Planes, lead: int = 0) -> None:
+    """srcs: 1-2 tuples (tensor, nhwc: bool); `lead` zero channels, then the sources' channels concatenated,
+    zero-filled to dst.c, written to dst and its twin in one pass.  Replaces cat((zeros, a, b), 1) + the channel
+    padding of the operand."""
+    assert 1 <= len(srcs) <= 2 and dst.c % 8 == 0 and dst.c_off % 8 == 0 and lead >= 0
+    args = [lead]
     for t, nhwc in srcs:
         ptr, layout, pitch, c, nhw = _src_args(t, nhwc)
         args += [ptr, layout, pitch, c]
