@@ -531,6 +531,26 @@ int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double
 /* dx[b, p, ch] (+)= sum_j m[b*c + ch][j] X_j[p]  — the style-loss gradient w.r.t. the raw image; dx NHWC fp32. */
 int sn_gram_bwd(const float* m, const float* src, long long s_n, long long s_c, long long s_p, int n, int c,
                 long long npix, float* dx, int dx_pitch, int accumulate, void* stream);
+/* Row blocks of a Gram matrix of any size (the style term over every rank's samples, or over more than 96 rows):
+ * out: double [n_a*c][n_b*c] (zeroed here) = A B^T, the rows of A read as in sn_gram from a (strides a_n, a_c, a_p; n_a
+ * samples), those of B from b (n_b >= n_a samples).  fp32 sums over each 128-pixel chunk, fp64 from there on. */
+int sn_gram_rows(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b, long long b_n,
+                 long long b_c, long long b_p, int n_b, int c, long long npix, double* out, void* stream);
+/* deterministic variant: the pixel splits' partial blocks in `slots` (sn_gram_rows_det_slots(n_a*c, n_b*c) doubles are
+ * enough), added in split order */
+int sn_gram_rows_det(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b,
+                     long long b_n, long long b_c, long long b_p, int n_b, int c, long long npix, double* out,
+                     double* slots, long long slots_cap, void* stream);
+long long sn_gram_rows_det_slots(int rows_l, int rows);
+/* For a [rows_l][rows] row block of the Gram matrices: *loss_acc += weight * sum((gram_out - gram_tgt)^2) / rows^2
+ * (this block's share of weight * MSELoss over the whole [rows][rows] matrices);  m = gscale * (d/d(gram_out) + transpose)
+ * on those rows (fp32).  One block: deterministic.  rows_l = rows, gscale = 1 gives sn_gram_mse's bits. */
+int sn_gram_rows_mse(const double* gram_out, const double* gram_tgt, int rows_l, int rows, double weight,
+                     double gscale, double* loss_acc, float* m, void* stream);
+/* dx[b, p, ch] (+)= sum_j m[b*c + ch][j] X_j[p] for the rows_l rows of m (whole samples b < rows_l / c) and the n*c
+ * rows X_j of src (strides as in sn_gram); dx NHWC fp32 [rows_l / c][npix][dx_pitch]. */
+int sn_gram_rows_bwd(const float* m, int rows_l, const float* src, long long s_n, long long s_c, long long s_p, int n,
+                     int c, long long npix, float* dx, int dx_pitch, int accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * ROIAlign + channel repack (swapnet_modules.py:209-240, torchvision roi_align aligned=False,

@@ -205,6 +205,11 @@ SIGNATURES = {
     "sn_feat_loss_fwd_bwd_det": (_I, [_VP, _I, _VP, _I, _LL, _I, C.c_double, C.c_double, _VP, _VP, _I, _VP, _LL, _VP]),
     "sn_gram_mse": (_I, [_VP, _VP, _I, C.c_double, _VP, _VP, _VP]),
     "sn_gram_bwd": (_I, [_VP, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _I, _I, _VP]),
+    "sn_gram_rows": (_I, [_VP, _LL, _LL, _LL, _I, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP]),
+    "sn_gram_rows_det": (_I, [_VP, _LL, _LL, _LL, _I, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP, _LL, _VP]),
+    "sn_gram_rows_det_slots": (_LL, [_I, _I]),
+    "sn_gram_rows_mse": (_I, [_VP, _VP, _I, _I, C.c_double, C.c_double, _VP, _VP, _VP]),
+    "sn_gram_rows_bwd": (_I, [_VP, _I, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _I, _I, _VP]),
     "sn_roi_align_pack_fwd": (_I, [_VP, _I, _I, _I, _I, _VP, _I, _I, _VP, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_tap_gemm_simt": (_I, [C.POINTER(SnTapGemmDesc), _VP]),
     "sn_pixel_fwd_stats": (_I, [C.POINTER(SnPixelDesc), _VP]),

@@ -345,6 +345,151 @@ __global__ void __launch_bounds__(kThreads) gram_bwd_kernel(const float* __restr
   }
 }
 
+// ---------------------------------------------------------------------------------
+// Row blocks of a Gram matrix with any number of rows: the style term over every rank's samples, or over more than
+// kGramMaxR rows on one GPU.  out[i][j] = sum_p A_i[p] B_j[p] for the R_l rows of A and the R rows of B, each row
+// r = (b, ch) read as in gram_kernel.  Nothing is sized by the row count: the output is cut into kRowT x kRowT tiles
+// (blockIdx.x) and the pixel chunks are split over blockIdx.y.  Each 128-pixel chunk is summed in fp32 as in
+// gram_kernel; the chunk sums are added in fp64, so an entry's fp32 chain is one chunk long whatever the split.
+// ---------------------------------------------------------------------------------
+constexpr int kRowT = 32;                      // rows per tile edge
+constexpr int kRowBlocks = 4 * SN_NUM_SMS;     // target block count of gram_rows / gram_rows_bwd
+
+struct RowSrc {
+  const float* p;
+  long long sn, sc, sp;
+};
+
+// tile[r][0:kGramP] <- rows r0 .. r0 + nr - 1 of s over pixels [p0, p0 + kGramP); zero past nr rows and npix pixels
+__device__ __forceinline__ void load_row_tile(float* tile, const RowSrc& s, int C, int r0, int nr, long long p0,
+                                              long long npix) {
+  constexpr int TP = kGramP + 1;
+  for (int i = threadIdx.x; i < kRowT * kGramP; i += blockDim.x) {
+    int r, p;
+    if (s.sp == 1) { r = i / kGramP; p = i - r * kGramP; } else { p = i / kRowT; r = i - p * kRowT; }
+    float v = 0.f;
+    if (r < nr && p0 + p < npix) {
+      const int g = r0 + r, b = g / C, c = g - b * C;
+      v = s.p[b * s.sn + c * s.sc + (p0 + p) * s.sp];
+    }
+    tile[r * TP + p] = v;
+  }
+}
+
+// Thread t owns the entries (i0 + t/16 + 16u, j0 + t%16 + 16v), u, v in {0, 1}.
+// DET: the block's partials go to slots[blockIdx.y][R_l * R] (det_sum_slots adds the pixel splits in order)
+template <bool DET>
+__global__ void __launch_bounds__(kThreads) gram_rows_kernel(RowSrc a, RowSrc b, int C, int Rl, int R,
+                                                              long long npix, double* __restrict__ out,
+                                                              double* __restrict__ slots) {
+  constexpr int TP = kGramP + 1;
+  __shared__ float ta[kRowT * TP], tb[kRowT * TP];
+  const int tiles_j = (R + kRowT - 1) / kRowT;
+  const int i0 = (blockIdx.x / tiles_j) * kRowT, j0 = (blockIdx.x % tiles_j) * kRowT;
+  const int ni = min(kRowT, Rl - i0), nj = min(kRowT, R - j0);
+  const int ti = threadIdx.x >> 4, tj = threadIdx.x & 15;
+  double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
+  const long long nchunks = (npix + kGramP - 1) / kGramP;
+  for (long long ch = blockIdx.y; ch < nchunks; ch += gridDim.y) {
+    const long long p0 = ch * kGramP;
+    __syncthreads();
+    load_row_tile(ta, a, C, i0, ni, p0, npix);
+    load_row_tile(tb, b, C, j0, nj, p0, npix);
+    __syncthreads();
+    const float* a0 = ta + ti * TP;
+    const float* a1 = ta + (ti + 16) * TP;
+    const float* b0 = tb + tj * TP;
+    const float* b1 = tb + (tj + 16) * TP;
+    float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;
+#pragma unroll 8
+    for (int p = 0; p < kGramP; ++p) {
+      const float x0 = a0[p], x1 = a1[p], y0 = b0[p], y1 = b1[p];
+      s00 += x0 * y0; s01 += x0 * y1; s10 += x1 * y0; s11 += x1 * y1;
+    }
+    acc[0][0] += (double)s00; acc[0][1] += (double)s01; acc[1][0] += (double)s10; acc[1][1] += (double)s11;
+  }
+#pragma unroll
+  for (int u = 0; u < 2; ++u)
+#pragma unroll
+    for (int v = 0; v < 2; ++v) {
+      const int i = ti + 16 * u, j = tj + 16 * v;
+      if (i < ni && j < nj) {
+        const long long idx = (long long)(i0 + i) * R + j0 + j;
+        if constexpr (DET) slots[(long long)blockIdx.y * Rl * R + idx] = acc[u][v];
+        else atomicAdd(&out[idx], acc[u][v]);
+      }
+    }
+}
+
+// loss_acc += weight * sum((Go - Gt)^2) / R^2 over an [R_l][R] row block;  M = 4 * weight * gscale * (Go - Gt) / R^2
+// (= gscale * (dL/dGo + its transpose) on those rows, the Gram matrices being symmetric).  gram_mse_kernel's arithmetic:
+// with R_l = R and gscale = 1 both give the same bits.
+__global__ void gram_rows_mse_kernel(const double* __restrict__ Go, const double* __restrict__ Gt, long long n, int R,
+                                     double weight, double gscale, double* __restrict__ loss_acc,
+                                     float* __restrict__ M) {
+  __shared__ double red[kThreads];
+  double l = 0.0;
+  const double inv = 1.0 / ((double)R * R);
+  const double mw = 4.0 * weight * gscale;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+    const double d = Go[i] - Gt[i];
+    l += d * d;
+    M[i] = (float)(mw * d * inv);
+  }
+  red[threadIdx.x] = l;
+  __syncthreads();
+  for (int o = kThreads / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) atomicAdd(loss_acc, weight * red[0] * inv);
+}
+
+// dx[b, p, ch] (+)= sum_j M[r][j] X_j[p] for the R_l rows r = b*C + ch of M and the R rows of X.  Block (x, y): row
+// tile y (kRowT rows of M), pixel chunks x, x + gridDim.x, ...; thread t owns pixel t % 128 of rows t/128 + 2k.
+// The columns j are summed in order in fp32 (the zero rows past R add exact zeros), as in gram_bwd_kernel.
+__global__ void __launch_bounds__(kThreads) gram_rows_bwd_kernel(const float* __restrict__ M, RowSrc x, int C, int Rl,
+                                                                  int R, long long npix, float* __restrict__ dx,
+                                                                  int pdx, int accumulate) {
+  constexpr int TP = kGramP + 1, MP = kRowT + 1, KR = kRowT / (kThreads / kGramP);
+  __shared__ float tx[kRowT * TP], tm[kRowT * MP];
+  const int i0 = blockIdx.y * kRowT;
+  const int p = threadIdx.x % kGramP, rg = threadIdx.x / kGramP;
+  const long long nchunks = (npix + kGramP - 1) / kGramP;
+  for (long long ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
+    const long long p0 = ch * kGramP;
+    float s[KR];
+#pragma unroll
+    for (int k = 0; k < KR; ++k) s[k] = 0.f;
+    for (int j0 = 0; j0 < R; j0 += kRowT) {
+      __syncthreads();
+      load_row_tile(tx, x, C, j0, min(kRowT, R - j0), p0, npix);
+      for (int t = threadIdx.x; t < kRowT * kRowT; t += blockDim.x) {
+        const int i = t / kRowT, j = t - i * kRowT;
+        tm[i * MP + j] = (i0 + i < Rl && j0 + j < R) ? M[(long long)(i0 + i) * R + j0 + j] : 0.f;
+      }
+      __syncthreads();
+#pragma unroll 4
+      for (int j = 0; j < kRowT; ++j) {
+        const float xv = tx[j * TP + p];
+#pragma unroll
+        for (int k = 0; k < KR; ++k) s[k] += tm[(rg + 2 * k) * MP + j] * xv;
+      }
+    }
+    if (p0 + p < npix) {
+#pragma unroll
+      for (int k = 0; k < KR; ++k) {
+        const int r = i0 + rg + 2 * k;
+        if (r < Rl) {
+          const int b = r / C, c = r - b * C;
+          float* d = dx + ((long long)b * npix + p0 + p) * pdx + c;
+          *d = accumulate ? *d + s[k] : s[k];
+        }
+      }
+    }
+  }
+}
+
 }  // namespace
 
 #define LAUNCH_CHECK()                         \
@@ -514,6 +659,90 @@ int sn_gram_bwd(const float* m, const float* src, long long s_n, long long s_c, 
   long long chunks = (npix + kGramP - 1) / kGramP;
   const int grid = (int)(chunks < 592 ? chunks : 592);
   gram_bwd_kernel<<<grid, kThreads, smem, st>>>(m, src, s_n, s_c, s_p, c, R, npix, dx, dx_pitch, accumulate);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+// pixel splits of gram_rows: enough blocks for kRowBlocks whatever the tile count, at most one per chunk
+static long long gram_rows_splits(long long rows_l, long long rows) {
+  const long long tiles = ((rows_l + kRowT - 1) / kRowT) * ((rows + kRowT - 1) / kRowT);
+  const long long p = (kRowBlocks + tiles - 1) / tiles;
+  return p < 1 ? 1 : p;
+}
+
+static int gram_rows_impl(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b,
+                          long long b_n, long long b_c, long long b_p, int n_b, int c, long long npix, double* out,
+                          double* slots, long long slots_cap, cudaStream_t st) {
+  SN_REQUIRE(a && b && out, "null pointer");
+  SN_REQUIRE(n_a >= 1 && c >= 1 && npix >= 1 && n_a <= n_b, "gram_rows: 1 <= n_a <= n_b samples, c >= 1, npix >= 1");
+  SN_REQUIRE(a_n >= 1 && a_c >= 1 && a_p >= 1 && b_n >= 1 && b_c >= 1 && b_p >= 1, "gram_rows: strides must be >= 1");
+  const long long rl = (long long)n_a * c, r = (long long)n_b * c;
+  SN_REQUIRE(r <= (1 << 20), "gram_rows: %lld rows, at most %d supported", r, 1 << 20);
+  const long long tiles = ((rl + kRowT - 1) / kRowT) * ((r + kRowT - 1) / kRowT);
+  SN_REQUIRE(tiles < (1LL << 31), "gram_rows: %lld output tiles", tiles);
+  const long long chunks = (npix + kGramP - 1) / kGramP;
+  long long splits = gram_rows_splits(rl, r);
+  if (splits > chunks) splits = chunks;
+  SN_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * rl * r, st));
+  const dim3 grid((unsigned)tiles, (unsigned)splits);
+  const RowSrc sa{a, a_n, a_c, a_p}, sb{b, b_n, b_c, b_p};
+  if (!slots) {
+    gram_rows_kernel<false><<<grid, kThreads, 0, st>>>(sa, sb, c, (int)rl, (int)r, npix, out, nullptr);
+    LAUNCH_CHECK();
+    return SN_OK;
+  }
+  SN_REQUIRE(splits * rl * r <= slots_cap, "gram_rows_det: %lld slots needed, %lld given", splits * rl * r, slots_cap);
+  gram_rows_kernel<true><<<grid, kThreads, 0, st>>>(sa, sb, c, (int)rl, (int)r, npix, out, slots);
+  LAUNCH_CHECK();
+  SN_CHECK_CUDA(det_sum_slots(slots, (int)splits, rl * r, out, st));
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_gram_rows(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b, long long b_n,
+                 long long b_c, long long b_p, int n_b, int c, long long npix, double* out, void* stream) {
+  return gram_rows_impl(a, a_n, a_c, a_p, n_a, b, b_n, b_c, b_p, n_b, c, npix, out, nullptr, 0, (cudaStream_t)stream);
+}
+
+int sn_gram_rows_det(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b,
+                     long long b_n, long long b_c, long long b_p, int n_b, int c, long long npix, double* out,
+                     double* slots, long long slots_cap, void* stream) {
+  SN_REQUIRE(slots, "gram_rows_det: null slots");
+  return gram_rows_impl(a, a_n, a_c, a_p, n_a, b, b_n, b_c, b_p, n_b, c, npix, out, slots, slots_cap,
+                        (cudaStream_t)stream);
+}
+
+long long sn_gram_rows_det_slots(int rows_l, int rows) {
+  if (rows_l < 1 || rows < 1) return 0;
+  return gram_rows_splits(rows_l, rows) * rows_l * rows;
+}
+
+int sn_gram_rows_mse(const double* gram_out, const double* gram_tgt, int rows_l, int rows, double weight,
+                     double gscale, double* loss_acc, float* m, void* stream) {
+  SN_REQUIRE(gram_out && gram_tgt && loss_acc && m, "null pointer");
+  SN_REQUIRE(rows_l >= 1 && rows_l <= rows, "gram_rows_mse: 1 <= rows_l (%d) <= rows (%d)", rows_l, rows);
+  gram_rows_mse_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(gram_out, gram_tgt, (long long)rows_l * rows, rows,
+                                                                  weight, gscale, loss_acc, m);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+int sn_gram_rows_bwd(const float* m, int rows_l, const float* src, long long s_n, long long s_c, long long s_p, int n,
+                     int c, long long npix, float* dx, int dx_pitch, int accumulate, void* stream) {
+  SN_REQUIRE(m && src && dx, "null pointer");
+  SN_REQUIRE(n >= 1 && c >= 1 && npix >= 1, "gram_rows_bwd: n, c, npix >= 1");
+  SN_REQUIRE(s_n >= 1 && s_c >= 1 && s_p >= 1 && dx_pitch >= c, "gram_rows_bwd: strides >= 1, dx_pitch >= c");
+  const long long r = (long long)n * c;
+  SN_REQUIRE(rows_l >= 1 && rows_l <= r && rows_l % c == 0,
+             "gram_rows_bwd: rows_l = %d must be whole samples of the %lld rows of src", rows_l, r);
+  SN_REQUIRE(r <= (1 << 20), "gram_rows_bwd: %lld rows, at most %d supported", r, 1 << 20);
+  const int row_tiles = (rows_l + kRowT - 1) / kRowT;
+  const long long chunks = (npix + kGramP - 1) / kGramP;
+  long long gx = (kRowBlocks + row_tiles - 1) / row_tiles;
+  if (gx > chunks) gx = chunks;
+  const RowSrc sx{src, s_n, s_c, s_p};
+  gram_rows_bwd_kernel<<<dim3((unsigned)gx, (unsigned)row_tiles), kThreads, 0, (cudaStream_t)stream>>>(
+      m, sx, c, rows_l, (int)r, npix, dx, dx_pitch, accumulate);
   LAUNCH_CHECK();
   return SN_OK;
 }

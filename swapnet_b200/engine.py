@@ -795,12 +795,20 @@ class PerceptualEngine:
 
     content = sum over 5 taps of MSE(f_out, f_tgt), f = L2-normalised ReLU features of `2x - 1`;
     style   = 5 * MSE(gram(out), gram(tgt)) of the raw images viewed as [B*3, H*W] (perceptual.py:58-63).
+
+    The style term has two device paths.  Up to 96 rows on one rank, `gram` / `gram_mse` / `gram_bwd` hold the whole
+    Gram matrix in one block's registers and shared memory.  Beyond that, or with a style exchange (`--b200_sync_style 1`
+    under data parallelism), the row kernels compute this rank's [R_l, R] row block of a Gram matrix of any size.
     """
 
+    KGRAM_MAX_ROWS = 96     # csrc/perceptual.cu kGramMaxR: the most rows `gram` / `gram_bwd` accept
+
     def __init__(self, net: Optional[M.VGG16Features], batch: int, size: int, device, nsplit: int = 3,
-                 content: bool = True, deterministic: bool = False):
+                 content: bool = True, deterministic: bool = False, style_exchange=None):
         """deterministic: the content and style sums add their block partials in a fixed order (bit-identical runs);
-        the VGG passes themselves have no cross-block reductions."""
+        the VGG passes themselves have no cross-block reductions.
+        style_exchange: a parallel.BNStatsExchange whose group the style term gathers every rank's fakes and targets
+        over, so that its Gram matrices are those of the whole batch; None (or one rank): this rank's samples only."""
         dev = torch.device(device)
         self.det_ws = ops.DetWorkspace(dev) if deterministic else None
         self.batch, self.size = batch, size
@@ -810,13 +818,21 @@ class PerceptualEngine:
             self.out = VGGEngine(net, batch, size, device, nsplit, backward=True)
             self.tgt = VGGEngine(net, batch, size, device, nsplit, backward=False)
             self.gfeat = [torch.zeros_like(s.y) for s in self.out.taps]
-        r = 3 * batch
-        if r > 96:   # csrc/perceptual.cu kGramMaxR: the Gram matrix of the style term is held in registers / smem
-            raise NotImplementedError(f"style loss: the Gram matrix couples 3 x batch = {r} rows, at most 96 are "
-                                      "supported per GPU (batch <= 32); use --lambda_style 0 or a smaller per-GPU batch")
-        self.gram_o = torch.zeros(r, r, dtype=torch.float64, device=dev)
-        self.gram_t = torch.zeros(r, r, dtype=torch.float64, device=dev)
-        self.gram_m = torch.zeros(r, r, dtype=torch.float32, device=dev)
+        ex = style_exchange if style_exchange is not None and style_exchange.world > 1 else None
+        self.style_exchange = ex
+        world = 1 if ex is None else ex.world
+        rl = 3 * batch
+        r = rl * world
+        self.rows_l, self.rows = rl, r
+        self.row_path = ex is not None or r > self.KGRAM_MAX_ROWS
+        self.gram_o = torch.zeros(rl, r, dtype=torch.float64, device=dev)
+        self.gram_t = torch.zeros(rl, r, dtype=torch.float64, device=dev)
+        self.gram_m = torch.zeros(rl, r, dtype=torch.float32, device=dev)
+        if ex is not None:     # every rank's samples in rank order, this rank's loss partial and all of them
+            self.fakes_all = torch.zeros(world * batch, size, size, 3, device=dev)
+            self.targets_all = torch.zeros(world * batch, 3, size, size, device=dev)
+            self.style_part = torch.zeros(1, dtype=torch.float64, device=dev)
+            self.style_parts = torch.zeros(world, dtype=torch.float64, device=dev)
 
     def workspace_bytes(self) -> int:
         """Device bytes of the deterministic mode's slot workspace (0 in the default mode)."""
@@ -851,8 +867,32 @@ class PerceptualEngine:
 
     def style(self, fakes: torch.Tensor, targets: torch.Tensor, lam: float, acc: torch.Tensor,
               grad_accum: torch.Tensor) -> None:
-        """acc += lam * 5 * MSE(gram(fakes), gram(targets)); grad_accum [B,S,S,3] += its gradient."""
-        ops.gram(fakes, True, self.gram_o, ws=self.det_ws)
-        ops.gram(targets, False, self.gram_t, ws=self.det_ws)
-        ops.gram_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
-        ops.gram_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)
+        """acc += lam * 5 * MSE(gram(fakes), gram(targets)); grad_accum [B,S,S,3] += its gradient.
+        With a style exchange: the Gram matrices of every rank's samples; acc receives the full-batch loss (the same
+        bits on every rank) and grad_accum `world` times the full-batch gradient w.r.t. this rank's fakes."""
+        ex = self.style_exchange
+        if not self.row_path:
+            ops.gram(fakes, True, self.gram_o, ws=self.det_ws)
+            ops.gram(targets, False, self.gram_t, ws=self.det_ws)
+            ops.gram_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
+            ops.gram_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)
+            return
+        if ex is None:       # one rank, more rows than `gram` holds: the whole matrix as one row block
+            ops.gram_rows(fakes, fakes, True, self.gram_o, ws=self.det_ws)
+            ops.gram_rows(targets, targets, False, self.gram_t, ws=self.det_ws)
+            ops.gram_rows_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
+            ops.gram_rows_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)
+            return
+        fa = ex.gather(fakes, self.fakes_all)
+        ta = ex.gather(targets, self.targets_all)
+        ops.gram_rows(fakes, fa, True, self.gram_o, ws=self.det_ws)       # rows of this rank x rows of all ranks
+        ops.gram_rows(targets, ta, False, self.gram_t, ws=self.det_ws)
+        self.style_part.zero_()
+        # m is scaled by `world`: the optimizer multiplies the summed G gradients by 1/world (BaseGAN.grad_scale),
+        # because every other term is a mean over the rank's shard and so world times its share of the full-batch
+        # gradient.  m @ X_all already is the full-batch gradient w.r.t. this rank's fakes, not a shard mean.
+        ops.gram_rows_mse(self.gram_o, self.gram_t, 5.0 * lam, self.style_part, self.gram_m, gscale=float(ex.world))
+        ops.gram_rows_bwd(self.gram_m, fa, True, grad_accum, accumulate=True)
+        parts = ex.gather(self.style_part, self.style_parts)
+        for r in range(ex.world):         # rank order, on every rank: every rank reports the same bits
+            acc.add_(parts[r:r + 1])

@@ -20,6 +20,7 @@ import torch
 from .. import engine as E
 from .. import modules as M
 from .. import ops
+from .. import parallel
 from ..ops import GradSrc
 from .base_gan import BaseGAN
 from .base_model import LazyLoss
@@ -36,6 +37,11 @@ class TextureModel(BaseGAN):
             parser.add_argument("--lambda_style", type=float, default=1e-8, help="weight for style loss in final term")
             parser.add_argument("--b200_vgg", default="pretrained",
                                 help="VGG16 weights of the perceptual loss: pretrained | random[:seed] | <state_dict path>")
+            parser.add_argument("--b200_sync_style", type=int, default=0, choices=(0, 1),
+                                help="1: under data parallelism, the style loss's Gram matrices cover every rank's "
+                                     "samples (fakes and targets gathered each step), so it is the full batch's loss "
+                                     "and gradient; no effect on one GPU.  0: each rank's Gram matrices couple its own "
+                                     "samples only")
             parser.set_defaults(display_ncols=5)
         return parser
 
@@ -52,6 +58,11 @@ class TextureModel(BaseGAN):
             self.lam_style = float(getattr(opt, "lambda_style", 0))
             self.net_vgg = None
             self._eng_P = None
+            # --b200_sync_style 1: the style term's gathers go over the batch-norm exchange's process group (one of its
+            # own is created when no network has batch norm); every rank builds it here, in the same order
+            self._style_sync = None
+            if self.lam_style != 0 and getattr(opt, "b200_sync_style", 0) and self._world > 1:
+                self._style_sync = self._bn_sync if self._bn_sync is not None else parallel.BNStatsExchange()
             if self.lam_content != 0:
                 # the reference builds PerceptualLoss unconditionally (texture_model.py:68); the frozen VGG is
                 # only needed when the content term is on (the style term uses the raw images)
@@ -104,7 +115,8 @@ class TextureModel(BaseGAN):
         e = super()._build_engines(batch, size)
         if self.is_train and (self.lam_content != 0 or self.lam_style != 0):
             e["P"] = E.PerceptualEngine(self.net_vgg, batch, size, self.device, self.nsplit,
-                                        content=self.lam_content != 0, deterministic=self.deterministic)
+                                        content=self.lam_content != 0, deterministic=self.deterministic,
+                                        style_exchange=self._style_sync)
         return e
 
     def ensure_engines(self, batch, size):

@@ -1051,6 +1051,43 @@ def gram_bwd(m: torch.Tensor, x: torch.Tensor, nhwc: bool, dx: torch.Tensor, acc
                                   1 if accumulate else 0, _stream()))
 
 
+def gram_rows(a: torch.Tensor, b: torch.Tensor, nhwc: bool, out: torch.Tensor,
+              ws: Optional[DetWorkspace] = None) -> None:
+    """out [n_a*c, n_b*c] (float64) = A B^T: the rows (sample, channel) of `a` against those of `b` (same layout and
+    image size; b may hold more samples, e.g. every rank's).  Any number of rows."""
+    na, c, npix, an, ac, ap = _gram_strides(a, nhwc)
+    nb, cb, npix_b, bn, bc, bp = _gram_strides(b, nhwc)
+    assert (cb, npix_b) == (c, npix) and out.dtype == torch.float64 and out.shape == (na * c, nb * c)
+    assert out.is_contiguous()
+    args = (a.data_ptr(), an, ac, ap, na, b.data_ptr(), bn, bc, bp, nb, c, npix, out.data_ptr())
+    if ws is not None:
+        sl = ws.get(int(_lib.load().sn_gram_rows_det_slots(na * c, nb * c)))
+        check(_lib.load().sn_gram_rows_det(*args, sl.data_ptr(), sl.numel(), _stream()))
+        return
+    check(_lib.load().sn_gram_rows(*args, _stream()))
+
+
+def gram_rows_mse(g_out: torch.Tensor, g_tgt: torch.Tensor, weight: float, loss_acc: torch.Tensor, m: torch.Tensor,
+                  gscale: float = 1.0) -> None:
+    """For [R_l, R] row blocks: loss_acc += weight * sum((g_out - g_tgt)^2) / R^2; m (fp32 [R_l, R]) = gscale *
+    (d/d g_out + transpose) on those rows."""
+    rows_l, rows = g_out.shape
+    assert g_tgt.shape == g_out.shape and m.dtype == torch.float32 and m.shape == g_out.shape
+    assert g_out.is_contiguous() and g_tgt.is_contiguous() and m.is_contiguous() and loss_acc.dtype == torch.float64
+    check(_lib.load().sn_gram_rows_mse(g_out.data_ptr(), g_tgt.data_ptr(), rows_l, rows, weight, gscale,
+                                       loss_acc.data_ptr(), m.data_ptr(), _stream()))
+
+
+def gram_rows_bwd(m: torch.Tensor, x: torch.Tensor, nhwc: bool, dx: torch.Tensor, accumulate: bool) -> None:
+    """dx (NHWC fp32 [R_l/c, h, w, >=c]) (+)= m @ X, m [R_l, n*c] against the n*c rows X of x."""
+    n, c, npix, sn, sc, sp = _gram_strides(x, nhwc)
+    rows_l = m.shape[0]
+    assert m.dtype == torch.float32 and m.is_contiguous() and m.shape[1] == n * c
+    assert dx.shape[0] * c == rows_l and dx.shape[1] * dx.shape[2] == npix
+    check(_lib.load().sn_gram_rows_bwd(m.data_ptr(), rows_l, x.data_ptr(), sn, sc, sp, n, c, npix, dx.data_ptr(),
+                                       _pitch(dx), 1 if accumulate else 0, _stream()))
+
+
 # ---------------------------------------------------------------------------------------------
 # one-output-channel conv helpers (csrc/patch_logits.cu)
 # ---------------------------------------------------------------------------------------------

@@ -5,7 +5,9 @@ ROIAlign and the batch-mean losses are all per-sample, so equal shards + gradien
 reproduce the single-process gradient (SURVEY §8e).  The only exchange step is one all-reduce of
 the flat fp32 gradient buffer per optimizer step; the smooth-label scalars (one draw per loss call
 for the whole batch, loss.py:65-77) come from an identically seeded generator on every rank.  Batch norm couples the
-samples of a call: with `--b200_sync_bn 1` its statistics are exchanged per call (BNStatsExchange).
+samples of a call: with `--b200_sync_bn 1` its statistics are exchanged per call (BNStatsExchange).  The texture
+stage's style loss couples every pair of samples: with `--b200_sync_style 1` the fakes and targets are gathered over the
+same exchange each step (engine.PerceptualEngine.style).
 """
 from __future__ import annotations
 
