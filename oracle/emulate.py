@@ -5,7 +5,12 @@
 Used by tests/ to (a) prove on the CPU that swapnet_b200/lowering.py maps every reference conv
 layer (modules/layers.py:15,31,131-138; swapnet_modules.py:85-90; discriminators.py:111-131)
 and its autograd onto those contractions exactly, and (b) check the CUDA kernels against the
-same spec on the GPU.  Nothing under swapnet_b200/ imports this file.
+same spec on the GPU: the single-pass (nsplit = 1) GEMMs are held to the fp64 contraction of the
+16-bit operands they read, computed here on the device (tests/test_kernels_gpu.py model_forward /
+model_dgrad / model_wgrad, used by test_conv_forward, test_conv_backward,
+test_conv_baseline_shapes_fwd_bwd and test_fused_instance_norm_statistics; by
+tests/test_gemm_edges_gpu.py and tests/test_deterministic_gpu.py::test_wgrad_plan_repeats_bit_identically;
+and directly by tests/test_single_pass_gemm_gpu.py).  Nothing under swapnet_b200/ imports this file.
 """
 from __future__ import annotations
 
@@ -19,8 +24,8 @@ def gather_patch(A: torch.Tensor, parity: bool, m_h: int, m_w: int, tap: L.Tap, 
     """A: [N, H, W, pitch] dense.  Returns [N, m_h, m_w, k] with zero for out-of-range pixels."""
     N, H, W, _ = A.shape
     out = A.new_zeros(N, m_h, m_w, k)
-    hs = torch.arange(m_h) + tap.dh
-    ws = torch.arange(m_w) + tap.dw
+    hs = torch.arange(m_h, device=A.device) + tap.dh
+    ws = torch.arange(m_w, device=A.device) + tap.dw
     if parity:
         vh = (hs >= 0) & (hs < H // 2)
         vw = (ws >= 0) & (ws < W // 2)

@@ -14,6 +14,7 @@ pytestmark = pytest.mark.gpu
 
 from test_engine_gpu import (_opt, _texture_step_vs_oracle, _warp_step_vs_oracle, dev, record, relmax,  # noqa: E402
                              synth_texture_batch, synth_warp_batch)
+from test_kernels_gpu import SP_SEP_BF16, at_both_nsplits, check_single_pass, model_wgrad  # noqa: E402
 
 
 @contextlib.contextmanager
@@ -89,42 +90,105 @@ def _differences(a, b):
     return f"{nl} of {len(la)} loss vectors and {nt} of {len(sa)} tensors differ, max |diff| {dmax:.2e}"
 
 
+def _conv_layers(model):
+    """Every conv layer of every engine of a model: G, Dd, Dg and, for the perceptual loss, both VGG16 engines."""
+    from swapnet_b200 import engine as E
+
+    engines = {}
+    for key, e in model._eng_extra.items():
+        if isinstance(e, E.PerceptualEngine):
+            engines.update({f"{key}.out": e.out, f"{key}.tgt": e.tgt})
+        elif isinstance(e, E.Engine):
+            engines[key] = e
+    return {f"{k}.{s.name}": s.layer for k, e in engines.items() if e is not None for s in e.stages}
+
+
+def _check_bf16_precision(case, run, mk, batch):
+    """`--b200_precision bf16`: every conv layer of every engine runs single-pass (an engine that ignored the option
+    would run nsplit = 3), one step's losses and gradients are finite and its losses within 1e-2 of the fp32x3 step's.
+    The gradients' distance from fp32x3 is recorded, not asserted: a 2^-8 operand rounding flips LeakyReLU and max-pool
+    gates, which spreads it over 1e-2 .. 1e-1 (DESIGN.md section 2)."""
+    from swapnet_b200.layers import ConvLayer
+
+    layers = _conv_layers(run[2])
+    convs = {k: ly for k, ly in layers.items() if isinstance(ly, ConvLayer)}
+    assert convs and all(ly.nsplit == 1 for ly in layers.values()), \
+        [k for k, ly in layers.items() if ly.nsplit != 1]
+    engines = sorted({k.split(".")[0] for k in convs})
+    assert engines == (["Dd", "Dg", "G", "P"] if "perceptual" in case else ["Dd", "Dg", "G"]), engines
+    one = {prec: _run(mk(1, prec), batch, 1) for prec in ("fp32x3", "bf16")}
+    lf, lb = one["fp32x3"][0][0], one["bf16"][0][0]
+    assert torch.isfinite(lb).all(), lb
+    assert (lb - lf).abs().max().item() <= 1e-2 * lf.abs().max().item(), (lb, lf)
+    rel = {}
+    for k in ("G.flat_grad", "D.flat_grad"):
+        gb, gf = one["bf16"][1][k], one["fp32x3"][1][k]
+        assert torch.isfinite(gb).all(), k
+        rel[k] = relmax(gb, gf)
+    record(f"bf16_precision_step_vs_fp32x3[{case}]", f"{len(convs)} conv layers at nsplit 1, losses max|diff| "
+           f"{(lb - lf).abs().max().item():.3e}, grads relmax " + " ".join(f"{k} {v:.3e}" for k, v in rel.items()))
+
+
 # ------------------------------------------------------------------------------------------------
 # whole steps
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", ["warp512", "texture_perceptual128", "texture_batchnorm128"])
-def test_identically_seeded_runs_are_bit_identical(case):
+@pytest.mark.parametrize("case,precision", [
+    pytest.param("warp512", "fp32x3", id="warp512"),
+    pytest.param("texture_perceptual128", "fp32x3", id="texture_perceptual128"),
+    pytest.param("texture_batchnorm128", "fp32x3", id="texture_batchnorm128"),
+    pytest.param("warp512", "bf16", id="warp512-bf16"),
+    pytest.param("texture_perceptual128", "bf16", id="texture_perceptual128-bf16"),
+])
+def test_identically_seeded_runs_are_bit_identical(case, precision):
     """Four steps (two eager, two graph replays) at the default learning rates: every loss, parameter, AdamW moment,
-    BatchNorm buffer and gradient is bit-identical between two fresh, identically seeded models."""
+    BatchNorm buffer and gradient is bit-identical between two fresh, identically seeded models.  With
+    `--b200_precision bf16` too (the default PatchGAN and the VGG16 perceptual engines single-pass)."""
     if case == "warp512":
         B, S = 2, 512
-        batch, mk = _warp_batch(B, S), lambda det: _opt(B, S, b200_deterministic=det)
+        batch = _warp_batch(B, S)
+        mk = lambda det, prec=precision: _opt(B, S, b200_deterministic=det, b200_precision=prec)  # noqa: E731
     elif case == "texture_perceptual128":     # the texture model's default loss weights, seeded-random VGG16
         B, S = 2, 128
         batch = _texture_batch(B, S)
-        mk = lambda det: _texture_opt(B, S, lambda_content=20, lambda_style=1e-8, b200_vgg="random",  # noqa: E731
-                                      b200_deterministic=det)
+        mk = lambda det, prec=precision: _texture_opt(B, S, lambda_content=20, lambda_style=1e-8,  # noqa: E731
+                                                      b200_vgg="random", b200_deterministic=det, b200_precision=prec)
     else:
         B, S = 2, 128
-        batch, mk = _texture_batch(B, S), lambda det: _texture_opt(B, S, norm="batch", b200_deterministic=det)
+        batch = _texture_batch(B, S)
+        mk = lambda det, prec=precision: _texture_opt(B, S, norm="batch", b200_deterministic=det,  # noqa: E731
+                                                      b200_precision=prec)
     a = _run(mk(1), batch, 4)
     assert a[2].deterministic and len(a[2]._graphs) == 1
+    assert a[2].nsplit == (1 if precision == "bf16" else 3)
     b = _run(mk(1), batch, 4)
     _assert_identical(a, b, case)
+    if precision == "bf16":
+        _check_bf16_precision(case, a, mk, batch)
     del a, b
     # evidence: the default mode on the same setup
     c, d = _run(mk(0), batch, 4), _run(mk(0), batch, 4)
-    record(f"deterministic_default_mode_run_to_run[{case}]", _differences(c, d))
+    record(f"deterministic_default_mode_run_to_run[{case}{'' if precision == 'fp32x3' else ',' + precision}]",
+           _differences(c, d))
+
+
+def _graph_vs_eager(precision):
+    B, S = 2, 64
+    batch = _warp_batch(B, S)
+    g = _run(_opt(B, S, b200_graph=1, b200_deterministic=1, b200_precision=precision), batch, 5)
+    e = _run(_opt(B, S, b200_graph=0, b200_deterministic=1, b200_precision=precision), batch, 5)
+    assert len(g[2]._graphs) == 1 and not e[2]._graphs
+    assert g[2].nsplit == e[2].nsplit == (1 if precision == "bf16" else 3)
+    _assert_identical(g, e, f"graph vs eager ({precision})")
 
 
 def test_graph_replay_is_bit_identical_to_eager_steps():
     """With non-zero learning rates, five steps with b200_graph=1 (two eager, three replays) equal five eager steps."""
-    B, S = 2, 64
-    batch = _warp_batch(B, S)
-    g = _run(_opt(B, S, b200_graph=1, b200_deterministic=1), batch, 5)
-    e = _run(_opt(B, S, b200_graph=0, b200_deterministic=1), batch, 5)
-    assert len(g[2]._graphs) == 1 and not e[2]._graphs
-    _assert_identical(g, e, "graph vs eager")
+    _graph_vs_eager("fp32x3")
+
+
+def test_graph_replay_is_bit_identical_to_eager_steps_at_bf16_precision():
+    """The same with `--b200_precision bf16`: the single-pass plans replay bit for bit."""
+    _graph_vs_eager("bf16")
 
 
 def test_agrees_with_the_default_mode():
@@ -240,12 +304,13 @@ def _planes(n, h, w, c, fmt, g, scale=1.0):
     return p, src
 
 
-@pytest.mark.parametrize("kind,cin,cout,hw,n", [("conv4s2", 64, 64, 128, 4), ("conv4s2", 32, 64, 128, 2),
-                                                ("conv3r", 128, 16, 32, 2)])
-def test_wgrad_plan_repeats_bit_identically(kind, cin, cout, hw, n):
+@pytest.mark.parametrize("kind,cin,cout,hw,n,nsplit", at_both_nsplits([("conv4s2", 64, 64, 128, 4),
+                                                                        ("conv4s2", 32, 64, 128, 2),
+                                                                        ("conv3r", 128, 16, 32, 2)]))
+def test_wgrad_plan_repeats_bit_identically(kind, cin, cout, hw, n, nsplit):
     """A deterministic weight-gradient plan (split-K >= 8; two cases with the narrow grouped-Y layout) gives the same bits
     on every launch, stays within test_kernels_gpu's 1e-4 bound of the fp64 product, and within 1e-5 of the default
-    (atomic) plan."""
+    (atomic) plan.  Single-pass (nsplit = 1): within 1.5e-5 of the fp64 product of the bf16 operands it reads."""
     import torch.nn.functional as F
 
     from swapnet_b200 import lowering as L
@@ -260,7 +325,7 @@ def test_wgrad_plan_repeats_bit_identically(kind, cin, cout, hw, n):
     w = (torch.randn(cout, cin, 3 if kind == "conv3r" else 4, 3 if kind == "conv3r" else 4, generator=g) * 0.05).to(dev())
     outs = {}
     for det in (True, False):
-        ly = ConvLayer(kind, w, None, x, det_ws=ops.DetWorkspace(dev()) if det else None)
+        ly = ConvLayer(kind, w, None, x, nsplit=nsplit, det_ws=ops.DetWorkspace(dev()) if det else None)
         dyc = max(L.padc(cout), 64 if x.c < 64 else 16)
         dy, dysrc = _planes(n, ly.out_h, ly.out_w, dyc, ops.FMT_BF16, torch.Generator().manual_seed(5))
         gw = torch.zeros_like(w)
@@ -279,9 +344,15 @@ def test_wgrad_plan_repeats_bit_identically(kind, cin, cout, hw, n):
     yr = F.conv2d(xr, wr) if kind == "conv3r" else F.conv2d(xr, wr, stride=2, padding=1)
     (gw64,) = torch.autograd.grad(yr, wr, dyr)
     e64 = relmax(outs[True].cpu(), gw64)
-    record(f"det_wgrad[{kind},{cin},{cout},{hw}]", f"ksplit {ks}, y_chunk {y_chunk}, vs fp64 {e64:.2e}, "
-           f"vs default relmax {relmax(outs[True], outs[False]):.2e}")
-    assert e64 < 1e-4, e64
+    tag = f"det_wgrad[{kind},{cin},{cout},{hw}" + ("]" if nsplit == 3 else ",nsplit=1]")
+    if nsplit == 3:
+        record(tag, f"ksplit {ks}, y_chunk {y_chunk}, vs fp64 {e64:.2e}, "
+               f"vs default relmax {relmax(outs[True], outs[False]):.2e}")
+        assert e64 < 1e-4, e64
+    else:   # ly: the atomic plan's layer, bound to the same operand values
+        e_m, sep = check_single_pass(tag, outs[True], model_wgrad(ly), gw64, 1.5e-5, SP_SEP_BF16)
+        record(tag, f"ksplit {ks}, y_chunk {y_chunk}, vs operand model {e_m:.2e} (model vs exact {sep:.2e}), "
+               f"vs default relmax {relmax(outs[True], outs[False]):.2e}")
     assert relmax(outs[True], outs[False]) < 1e-5
     if kind == "conv4s2" and cin == 64:
         assert ks >= 8

@@ -9,7 +9,9 @@
 - the input-magnitude window of the fp16-split operands.
 
 References are fp64 torch on the GPU.  Bounds as in test_kernels_gpu: forward (fp16-split x3) 1.5e-5, backward
-(bf16-split x3) 1e-4, as max|err| / max|ref|.
+(bf16-split x3) 1e-4, as max|err| / max|ref|.  The schedule, repeat, split-K and fused-statistics tests also run every
+case single-pass (nsplit = 1, `--b200_precision bf16`: a 6-stage ring in place of 3), held to 1.5e-5 of the fp64
+product of the 16-bit operands the plan reads (test_kernels_gpu's operand model).
 """
 import ctypes
 
@@ -18,7 +20,8 @@ import torch
 import torch.nn.functional as F
 
 from swapnet_b200 import lowering as L
-from test_kernels_gpu import dev, make_layer, nhwc, record, ref_forward, ref_fwd_bwd, relmax
+from test_kernels_gpu import (SP_SEP_BF16, SP_SEP_FP16, at_both_nsplits, check_single_pass, dev, make_layer,
+                              model_forward, model_wgrad, nhwc, record, ref_forward, ref_fwd_bwd, relmax)
 
 pytestmark = pytest.mark.gpu
 
@@ -197,14 +200,14 @@ SCHEDULE_CASES = [
 ]
 
 
-@pytest.mark.parametrize("kind,cout,target", SCHEDULE_CASES)
-def test_tile_totals_around_sm_count(kind, cout, target):
+@pytest.mark.parametrize("kind,cout,target,nsplit", at_both_nsplits(SCHEDULE_CASES))
+def test_tile_totals_around_sm_count(kind, cout, target, nsplit):
     s = sm_count()
     want = {"1": 1, "s-1": s - 1, "s": s, "s+1": s + 1, "2s+1": 2 * s + 1}[target]
     per_image = (4 if kind == "convT4s2" else 1) * -(-cout // L.pick_block_n(cout))   # phases x N tiles
     n = -(-want // per_image)
     cin, h, w = 64, 8, 16
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     y = torch.full((n, oh, ow, cout), NAN, device=dev())
     layer.bind_forward(y)
@@ -214,9 +217,15 @@ def test_tile_totals_around_sm_count(kind, cout, target):
     layer.pack()
     layer.forward()
     torch.cuda.synchronize()
-    err = relmax(y, nhwc(ref_gpu(kind, x, wt, bias)))
-    record(f"tile_totals[{kind},{cin},{cout},n={n},tiles={tiles},sms={s}]", f"{err:.3e}")
-    assert err < FWD_TOL, err
+    exact = nhwc(ref_gpu(kind, x, wt, bias))
+    tag = f"tile_totals[{kind},{cin},{cout},n={n},tiles={tiles},sms={s}" + ("]" if nsplit == 3 else ",nsplit=1]")
+    if nsplit == 3:
+        err = relmax(y, exact)
+        record(tag, f"{err:.3e}")
+        assert err < FWD_TOL, err
+    else:
+        err, sep = check_single_pass(tag, y, model_forward(layer), exact, FWD_TOL, SP_SEP_FP16)
+        record(tag, f"{err:.3e} (model vs exact {sep:.3e})")
     assert not torch.isnan(y).any()
 
 
@@ -232,12 +241,12 @@ REPEAT_CASES = [
 ]
 
 
-@pytest.mark.parametrize("kind,n,cin,cout,h,w", REPEAT_CASES)
-def test_repeated_launches_bit_identical(kind, n, cin, cout, h, w):
+@pytest.mark.parametrize("kind,n,cin,cout,h,w,nsplit", at_both_nsplits(REPEAT_CASES))
+def test_repeated_launches_bit_identical(kind, n, cin, cout, h, w, nsplit):
     from swapnet_b200 import ops
 
     d = dev()
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     y = torch.empty(n, oh, ow, cout, device=d)
     stats = torch.empty(n, cout, 2, dtype=torch.float64, device=d) if kind == "conv3r" else None
@@ -255,12 +264,17 @@ def test_repeated_launches_bit_identical(kind, n, cin, cout, h, w):
             stats.fill_(NAN)
 
     def check_ref(xv, tag):
-        ref = ref_gpu(kind, xv, wt, bias)
-        err = relmax(y, nhwc(ref))
+        ref = nhwc(ref_gpu(kind, xv, wt, bias))
+        sep = ""
+        if nsplit == 1:   # against the operand model (the planes hold xv's 16-bit words)
+            model = model_forward(layer)
+            err, s_ = check_single_pass(f"repeat {tag}", y, model, ref, FWD_TOL, SP_SEP_FP16)
+            ref, sep = model, f" (model vs exact {s_:.3e})"
+        err = relmax(y, ref)
         e_s = 0.0
         if stats is not None:
-            e_s = max(relmax(stats[..., 0], ref.sum((2, 3))), relmax(stats[..., 1], (ref * ref).sum((2, 3))))
-        record(f"repeat[{kind},{n},{cin},{cout},{h}x{w},{tag}]", f"fwd {err:.3e} stats {e_s:.3e}")
+            e_s = max(relmax(stats[..., 0], ref.sum((1, 2))), relmax(stats[..., 1], (ref * ref).sum((1, 2))))
+        record(f"repeat[{kind},{n},{cin},{cout},{h}x{w},{tag},nsplit={nsplit}]", f"fwd {err:.3e} stats {e_s:.3e}{sep}")
         assert err < FWD_TOL and e_s < 1e-5, (tag, err, e_s)
 
     def check_same(tag):
@@ -299,7 +313,7 @@ def test_repeated_launches_bit_identical(kind, n, cin, cout, h, w):
     del g
 
     # beside a weight-gradient plan of another layer on a second stream (fork and join through events)
-    other, ox, owt, ob = make_layer("conv3r", 4, 128, 128, 32, 32, 3)
+    other, ox, owt, ob = make_layer("conv3r", 4, 128, 128, 32, 32, nsplit)
     ogy = torch.randn((4, 128, 32, 32), generator=torch.Generator().manual_seed(3)).to(d)
     _, _, ogw, _ = ref_fwd_bwd("conv3r", ox, owt, ob, ogy)
     owg = torch.zeros_like(other.weight)
@@ -319,9 +333,12 @@ def test_repeated_launches_bit_identical(kind, n, cin, cout, h, w):
     main.wait_event(join)
     torch.cuda.synchronize()
     check_same("beside a weight-gradient launch")
-    e_w = relmax(owg, ogw)
-    record(f"repeat[{kind},{n},{cin},{cout},{h}x{w},concurrent wgrad]", f"wgrad {e_w:.3e}")
-    assert e_w < BWD_TOL, e_w
+    if nsplit == 3:
+        e_w = relmax(owg, ogw)
+        assert e_w < BWD_TOL, e_w
+    else:
+        e_w, _ = check_single_pass("concurrent wgrad", owg, model_wgrad(other), ogw, FWD_TOL, SP_SEP_BF16)
+    record(f"repeat[{kind},{n},{cin},{cout},{h}x{w},concurrent wgrad,nsplit={nsplit}]", f"wgrad {e_w:.3e}")
 
 
 # ---------------------------------------------------------------------------------------------
@@ -340,12 +357,12 @@ WGRAD_CASES = [
 ]
 
 
-@pytest.mark.parametrize("kind,n,cin,cout,h,w,swap,rows,cols", WGRAD_CASES)
-def test_wgrad_split_k_accumulates(kind, n, cin, cout, h, w, swap, rows, cols):
+@pytest.mark.parametrize("kind,n,cin,cout,h,w,swap,rows,cols,nsplit", at_both_nsplits(WGRAD_CASES))
+def test_wgrad_split_k_accumulates(kind, n, cin, cout, h, w, swap, rows, cols, nsplit):
     from swapnet_b200 import ops
 
     d = dev()
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     gen = torch.Generator().manual_seed(99)
     gy = torch.randn((n, cout, oh, ow), generator=gen).to(d)
@@ -358,7 +375,7 @@ def test_wgrad_split_k_accumulates(kind, n, cin, cout, h, w, swap, rows, cols):
     s_row, s_col = L.wgrad_out_strides(kind, cin, cout, x_is_dy)
 
     def plan_for(out, ksplit):
-        desc = ops.wgrad_desc(xs, ys, ws, out, s_row, s_col, list(ws.tap_ids), cx, cy, swap=swap, nsplit=3,
+        desc = ops.wgrad_desc(xs, ys, ws, out, s_row, s_col, list(ws.tap_ids), cx, cy, swap=swap, nsplit=nsplit,
                               ksplit=ksplit)
         assert (desc.rows_valid, desc.cols_valid) == (rows, cols)
         assert (desc.ngroups > 0) == (min(xs.c, ys.c) < 64)
@@ -368,6 +385,11 @@ def test_wgrad_split_k_accumulates(kind, n, cin, cout, h, w, swap, rows, cols):
     probe = torch.zeros_like(layer.weight)
     total = geometry(plan_for(probe, 1 << 20)[0])[3]
     g0 = (torch.randn(wt.shape, generator=gen) * gw.abs().max().item()).float().to(d)
+    ref, tol, sep = gw, BWD_TOL, ""
+    if nsplit == 1:   # single pass: against the operand model, at the forward bound
+        ref, tol = model_wgrad(layer, dy), FWD_TOL
+        sep = f" model vs exact {relmax(ref, gw):.3e}"
+        assert relmax(ref, gw) >= SP_SEP_BF16 * tol
     outs, errs = {}, {}
     for ks in (1, 2, 3, 7, total, total + 5):
         out = g0.clone()
@@ -376,13 +398,13 @@ def test_wgrad_split_k_accumulates(kind, n, cin, cout, h, w, swap, rows, cols):
         plan.run()
         torch.cuda.synchronize()
         outs[ks] = out
-        errs[ks] = relmax(out.double() - g0.double(), gw)    # += into the torch-layout gradient
+        errs[ks] = relmax(out.double() - g0.double(), ref)    # += into the torch-layout gradient
     scale = gw.abs().max().item()
     spread = max((outs[k].double() - outs[1].double()).abs().max().item() / scale for k in outs)
     groups = [desc.group_size[i] for i in range(desc.ngroups)]
-    record(f"wgrad_split_k[{kind},{n},{cin},{cout},{h}x{w},swap={swap},tiles={total},groups={groups}]",
-           " ".join(f"k{k} {e:.3e}" for k, e in errs.items()) + f" spread {spread:.3e}")
-    assert max(errs.values()) < BWD_TOL, errs
+    record(f"wgrad_split_k[{kind},{n},{cin},{cout},{h}x{w},swap={swap},tiles={total},groups={groups},nsplit={nsplit}]",
+           " ".join(f"k{k} {e:.3e}" for k, e in errs.items()) + f" spread {spread:.3e}" + sep)
+    assert max(errs.values()) < tol, errs
     assert spread < SPLIT_SPREAD, spread
 
 

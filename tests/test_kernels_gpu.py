@@ -2,7 +2,9 @@
 restatements of the reference ops (and the numpy ROI oracle).
 
 Tolerances (max|err| / max|ref|; the north-star bar is 1e-3 relative fp32): forward GEMMs run
-fp16-split x3 -> < 1.5e-5; backward GEMMs run bf16-split x3 -> < 1e-4; single-pass fp16 < 5e-3.
+fp16-split x3 -> < 1.5e-5; backward GEMMs run bf16-split x3 -> < 1e-4.  Single-pass GEMMs (nsplit = 1,
+`--b200_precision bf16`) are held to 1.5e-5 (3e-5 at the baseline shapes) against the fp64 product of the
+16-bit operands they read (the operand model below).
 """
 import numpy as np
 import pytest
@@ -115,6 +117,130 @@ def make_layer(kind, n, cin, cout, h, w, nsplit, with_bias=True):
     return layer, x, wt, bias
 
 
+# ---------------------------------------------------------------------------------------------
+# the single-pass (nsplit = 1) operand model
+# ---------------------------------------------------------------------------------------------
+# A product of two 16-bit values is exact in fp32 (fp16 x fp16: 22 significant bits, bf16 x bf16: 16), so the only
+# error a correct single-pass GEMM may have is its fp32 accumulation.  Its reference is therefore the fp64 contraction
+# of the hi planes the plan reads, not of the fp32 tensors: decoded over the valid channels only (a pad channel counts
+# as zero, so garbage read from one shows up as an error) and contracted by oracle/emulate.py over the lowering's specs,
+# in fp64 on the device.
+#
+# Sensitivity: the distance of that model from the exact fp64 result is what the bound has to tell apart from the
+# single-pass result.  bf16 operands (backward GEMMs, unit roundoff 2^-8) put it at more than 20x the bound.  fp16
+# operands (forward, 2^-11) put it at 1.2e-4 .. 2.9e-4 whatever the shape: 8x .. 19x the 1.5e-5 bound of CONV_CASES
+# and 5x .. 9x the 3e-5 of the baseline shapes, so the forward asserts >= 4x the bound.  Every case also asserts that
+# the model is >= 20x farther from the exact result than the kernel is from the model.
+SP_SEP_BF16, SP_SEP_FP16 = 20.0, 4.0
+
+
+def hi_values(t, fmt):
+    """fp64 values of the hi words of a split 16-bit buffer (fp16 or bf16 bit patterns stored as bfloat16)."""
+    from swapnet_b200 import ops
+
+    return (t.view(torch.float16) if fmt == ops.FMT_F16 else t).double()
+
+
+def plane_hi(p, c):
+    """fp64 [n, h, w, p.c]: the hi plane of operand planes p, channels >= c zero."""
+    a = hi_values(p.hi[..., p.c_off:p.c_off + p.c], p.fmt).clone()
+    a[..., c:] = 0
+    return a
+
+
+def model_forward(layer):
+    """fp64 NHWC [n, out_h, out_w, cout]: the contraction of x.hi with the decoded packed weights wp.hi / wscale[0]
+    (the head's effective taps as the packer summed them), plus the bias."""
+    from oracle import emulate as E
+
+    kind, k, cout = layer.kind, layer.k_pad, layer.cout
+    a = plane_hi(layer.x, layer.cin)
+    wm = hi_values(layer.wp.hi, layer.wp.fmt) / layer.wscale[0].double()
+    b = None if layer.bias is None else layer.bias.double()
+    out = a.new_zeros(layer.n, layer.out_h, layer.out_w, cout)
+    if layer.stacked:   # one 9-shift contraction, the 4 output phases side by side along N
+        slot, spec = L.HEAD_SLOT, L.head_stacked_spec(layer.in_h, layer.in_w)
+        plain = L.GemmSpec(False, spec.m_h, spec.m_w, spec.taps, (1, 1), (0, 0), a_hw=spec.a_hw)
+        acc = a.new_zeros(layer.n, spec.m_h, spec.m_w, 4 * slot)
+        E.emul_tap_gemm(a, plain, wm, k, 4 * slot, acc)
+        for p in range(4):
+            out[:, p >> 1::2, p & 1::2] = acc[..., p * slot:p * slot + cout]
+        return out if b is None else out + b
+    for spec in L.forward_specs(kind, layer.in_h, layer.in_w):
+        w = wm
+        if kind == "head":   # per-phase matrices [rows_pad][ntaps_p * k] at HEAD_PHASE_OFF
+            p = spec.w_phase
+            nt = L.head_neff(p >> 1) * L.head_neff(p & 1)
+            off = layer.rows_pad * k * L.HEAD_PHASE_OFF[p]
+            w = wm.reshape(-1)[off:off + layer.rows_pad * nt * k].reshape(layer.rows_pad, nt * k)
+        E.emul_tap_gemm(a, spec, w, k, cout, out, bias=b)
+    return out
+
+
+def model_dgrad(layer):
+    """fp64 NHWC input gradient (over the padded grid for conv3r): dy.hi contracted with the bf16 pack wd.hi."""
+    from oracle import emulate as E
+
+    a = plane_hi(layer.dy, layer.cout)
+    wm = hi_values(layer.wd.hi, layer.wd.fmt)
+    ih, iw = (layer.in_h + 2, layer.in_w + 2) if layer.kind == "conv3r" else (layer.in_h, layer.in_w)
+    dx = a.new_zeros(layer.n, ih, iw, layer.cin)
+    for spec in L.dgrad_specs(layer.kind, layer.in_h, layer.in_w):
+        E.emul_tap_gemm(a, spec, wm, layer.dy.c, layer.cin, dx)
+    return dx
+
+
+def model_wgrad(layer, dy=None):
+    """fp64 weight gradient in torch layout: the hi planes of dy (default: the one bound to the layer) and of the bf16
+    twin of the input, contracted over the pixels (emul_wgrad), scattered through the plan's output strides and, for
+    the head, folded from effective taps."""
+    from oracle import emulate as E
+
+    kind, cin, cout = layer.kind, layer.cin, layer.cout
+    dy = layer.dy if dy is None else dy
+    (ws,) = L.wgrad_specs(kind, layer.in_h, layer.in_w)
+    x_is_dy = ws.x_is == "dy"
+    xin = layer.x if layer.x.fmt == dy.fmt else layer.x.twin
+    a, d = plane_hi(xin, cin), plane_hi(dy, cout)
+    xd, yd = (d, a) if x_is_dy else (a, d)
+    cx, cy = (cout, cin) if x_is_dy else (cin, cout)
+    g = E.emul_wgrad(xd, yd, ws, cx, cy)
+    s_row, s_col = L.wgrad_out_strides(kind, cin, cout, x_is_dy)
+    n_out = cout * 25 * cin if kind == "head" else layer.weight.numel()
+    tap_off = [t * cin for t in ws.tap_ids] if kind == "head" else list(ws.tap_ids)
+    flat = g.new_zeros(n_out)
+    rc = (torch.arange(cx, device=g.device)[:, None] * s_row + torch.arange(cy, device=g.device)[None, :] * s_col)
+    for t, off in enumerate(tap_off):
+        flat.index_add_(0, (rc + off).reshape(-1), g[t].reshape(-1))
+    if kind == "head":
+        return E.fold_head_wgrad_ref(flat.reshape(cout, 25, cin))
+    return flat.reshape(layer.weight.shape)
+
+
+def at_both_nsplits(cases):
+    """Parameter rows of a test over nsplit: every case at nsplit = 3 under the id it had before the nsplit = 1 rows
+    came, then every case at nsplit = 1 with '-nsplit1' appended; the last argument of the test is nsplit."""
+    rows = []
+    for ns in (3, 1):
+        for c in cases:
+            c = c if isinstance(c, tuple) else (c,)
+            cid = "-".join(str(v) for v in c)
+            rows.append(pytest.param(*c, ns, id=cid if ns == 3 else f"{cid}-nsplit1"))
+    return rows
+
+
+def check_single_pass(what, got, model, exact, tol, sep_factor):
+    """got within tol of the operand model, and the model far enough from the exact result that the bound tells the
+    single-pass result apart from it.  Returns (err, sep) for record()."""
+    model = model.to(got.device)
+    exact = exact.to(got.device)
+    err, sep = relmax(got, model), relmax(model, exact)
+    assert err < tol, f"{what}: relmax {err:.3e} vs the operand model (bound {tol:.1e})"
+    assert sep >= sep_factor * tol and sep >= 20 * err, \
+        f"{what}: model vs exact {sep:.3e} cannot separate the bound {tol:.1e} / the error {err:.3e}"
+    return err, sep
+
+
 @pytest.mark.parametrize("nsplit", [3, 1])
 @pytest.mark.parametrize("kind,n,cin,cout,h,w", CONV_CASES)
 def test_conv_forward(kind, n, cin, cout, h, w, nsplit):
@@ -129,12 +255,17 @@ def test_conv_forward(kind, n, cin, cout, h, w, nsplit):
     torch.cuda.synchronize()
     ref = nhwc(ref_forward(kind, x.double(), wt.double(), bias.double()))
     got = y[..., 2:2 + cout].cpu()
-    err = relmax(got, ref)
-    # fp16-split x3: operands carry 22 bits; what remains (~3e-6) is the tensor core's fp32
-    # accumulation (truncating adds).  Single-pass fp16 ~2^-11.
-    tol = 1.5e-5 if nsplit == 3 else 5e-3
-    record(f"conv_fwd[{kind},{n},{cin},{cout},{h}x{w},nsplit={nsplit}]", f"{err:.3e}")
-    assert err < tol, f"{kind} fwd nsplit={nsplit}: relmax {err:.3e}"
+    tag = f"conv_fwd[{kind},{n},{cin},{cout},{h}x{w},nsplit={nsplit}]"
+    if nsplit == 3:
+        # fp16-split x3: operands carry 22 bits; what remains (~3e-6) is the tensor core's fp32
+        # accumulation (truncating adds)
+        err = relmax(got, ref)
+        record(tag, f"{err:.3e}")
+        assert err < 1.5e-5, f"{kind} fwd nsplit={nsplit}: relmax {err:.3e}"
+    else:
+        # single pass: the same fp32-accumulation floor, against the fp64 product of the fp16 hi words it reads
+        err, sep = check_single_pass(tag, y[..., 2:2 + cout], model_forward(layer), ref, 1.5e-5, SP_SEP_FP16)
+        record(tag, f"{err:.3e} (model vs exact {sep:.3e})")
     assert torch.all(y[..., :2] == 7.0) and torch.all(y[..., 2 + cout:] == 7.0), "wrote outside its channel slice"
     if nsplit == 3 and not getattr(layer, "stacked", False):  # SIMT cross-check of the same descriptors (same split operands)
         y2 = torch.zeros_like(y)
@@ -152,11 +283,11 @@ def test_conv_forward(kind, n, cin, cout, h, w, nsplit):
         assert relmax(y2[..., 2:2 + cout].cpu(), ref) < 5e-6   # fp32 FMA chain over K up to 2048
 
 
-@pytest.mark.parametrize("kind,n,cin,cout,h,w", CONV_CASES)
-def test_conv_backward(kind, n, cin, cout, h, w):
+@pytest.mark.parametrize("kind,n,cin,cout,h,w,nsplit", at_both_nsplits(CONV_CASES))
+def test_conv_backward(kind, n, cin, cout, h, w, nsplit):
     from swapnet_b200 import ops
 
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     xr = x.double().requires_grad_()
     wr = wt.double().requires_grad_()
@@ -184,13 +315,21 @@ def test_conv_backward(kind, n, cin, cout, h, w):
     layer.pack()
     layer.backward()
     torch.cuda.synchronize()
-    e_dx = relmax(dx[..., 1:1 + cin].cpu(), nhwc(gx))
-    e_w = relmax(wg.cpu(), gw)
+    # the bias gradient is no GEMM: bias_grad_kernel reads hi + lo whatever nsplit is
     e_b = relmax(bg.cpu(), gb)
-    record(f"conv_bwd[{kind},{n},{cin},{cout},{h}x{w}]", f"dx {e_dx:.3e} w {e_w:.3e} b {e_b:.3e}")
-    assert e_dx < 1e-4, f"{kind} dgrad relmax {e_dx:.3e}"
-    assert e_w < 1e-4, f"{kind} wgrad relmax {e_w:.3e}"
     assert e_b < 1e-4, f"{kind} bias grad relmax {e_b:.3e}"
+    if nsplit == 3:
+        e_dx = relmax(dx[..., 1:1 + cin].cpu(), nhwc(gx))
+        e_w = relmax(wg.cpu(), gw)
+        record(f"conv_bwd[{kind},{n},{cin},{cout},{h}x{w}]", f"dx {e_dx:.3e} w {e_w:.3e} b {e_b:.3e}")
+        assert e_dx < 1e-4, f"{kind} dgrad relmax {e_dx:.3e}"
+        assert e_w < 1e-4, f"{kind} wgrad relmax {e_w:.3e}"
+    else:
+        e_dx, s_dx = check_single_pass(f"{kind} dgrad", dx[..., 1:1 + cin], model_dgrad(layer), nhwc(gx), 1.5e-5,
+                                       SP_SEP_BF16)
+        e_w, s_w = check_single_pass(f"{kind} wgrad", wg, model_wgrad(layer), gw, 1.5e-5, SP_SEP_BF16)
+        record(f"conv_bwd[{kind},{n},{cin},{cout},{h}x{w},nsplit=1]",
+               f"dx {e_dx:.3e} w {e_w:.3e} b {e_b:.3e} (model vs exact: dx {s_dx:.3e} w {s_w:.3e})")
     assert torch.all(dx[..., 0] == 5.0) and torch.all(dx[..., 1 + cin:] == 5.0)
 
 
@@ -231,11 +370,11 @@ def ref_fwd_bwd(kind, x, wt, bias, gy, chunk=4):
     return torch.cat(ys), torch.cat(gxs), gw, gb
 
 
-@pytest.mark.parametrize("kind,n,cin,cout,h,w", BASELINE_CASES)
-def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w):
+@pytest.mark.parametrize("kind,n,cin,cout,h,w,nsplit", at_both_nsplits(BASELINE_CASES))
+def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w, nsplit):
     from swapnet_b200 import ops
 
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     d = dev()
     y = torch.zeros(n, oh, ow, cout, device=d)
@@ -247,6 +386,9 @@ def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w):
         gy = torch.randn((n, cout, oh, ow), generator=torch.Generator().manual_seed(99)).to(d)
         yr, gx, gw, gb = ref_fwd_bwd(kind, x, wt, bias, gy)
         e_f = relmax(y, nhwc(yr))
+        if nsplit == 1:
+            e_f, s_f = check_single_pass(f"{kind} fwd", y, model_forward(layer), nhwc(yr), 3e-5, SP_SEP_FP16)
+        del yr
     dyc = L.padc(cout) if layer.x.c >= 64 else L.pad64(cout)
     dy = ops.Planes(n, oh, ow, dyc, d, fmt=ops.FMT_BF16)
     if cout * 33 * 4 > 48 * 1024:
@@ -261,7 +403,17 @@ def test_conv_baseline_shapes_fwd_bwd(kind, n, cin, cout, h, w):
     layer.pack()
     layer.backward()
     torch.cuda.synchronize()
-    e_dx, e_w, e_b = relmax(dx, nhwc(gx)), relmax(wg, gw), relmax(bg, gb)
+    e_b = relmax(bg, gb)
+    if nsplit == 1:   # the real K (up to 9216) and the 1 M-pixel weight-gradient reductions, single pass
+        e_dx, s_dx = check_single_pass(f"{kind} dgrad", dx, model_dgrad(layer), nhwc(gx), 3e-5, SP_SEP_BF16)
+        del gx
+        e_w, s_w = check_single_pass(f"{kind} wgrad", wg, model_wgrad(layer), gw, 3e-5, SP_SEP_BF16)
+        record(f"conv_baseline_shape[{kind},{n},{cin},{cout},{h}x{w},nsplit=1]",
+               f"fwd {e_f:.3e} dx {e_dx:.3e} w {e_w:.3e} b {e_b:.3e} "
+               f"(model vs exact: fwd {s_f:.3e} dx {s_dx:.3e} w {s_w:.3e})")
+        assert e_b < 1e-4, e_b
+        return
+    e_dx, e_w = relmax(dx, nhwc(gx)), relmax(wg, gw)
     record(f"conv_baseline_shape[{kind},{n},{cin},{cout},{h}x{w}]",
            f"fwd {e_f:.3e} dx {e_dx:.3e} w {e_w:.3e} b {e_b:.3e}")
     # forward: fp16-split x3 operands; the floor is the tensor core's truncating fp32 accumulator (grows with K).
@@ -701,18 +853,19 @@ def test_to_one_conv_layer(n, cin, h, w):
     assert e_y < 3e-5 and e_dx < 1e-4 and e_w < 1e-4 and e_b < 1e-4, (e_y, e_dx, e_w, e_b)
 
 
-@pytest.mark.parametrize("kind,n,cin,cout,h,w,fused", [("conv4s2", 2, 64, 128, 32, 64, True), ("convT4s2", 2, 128, 64, 16, 16, True),
-                                                     ("conv3r", 3, 128, 128, 32, 32, True), ("conv4s1", 2, 128, 256, 64, 64, True),
-                                                     ("conv4s2", 3, 128, 192, 16, 16, False),
-                                                     ("conv4s2", 2, 36, 36, 64, 64, False),   # n_valid % 16 != 0
-                                                     ("conv4s2", 2, 55, 64, 64, 64, True)])
-def test_fused_instance_norm_statistics(kind, n, cin, cout, h, w, fused):
+@pytest.mark.parametrize("kind,n,cin,cout,h,w,fused,nsplit", at_both_nsplits([
+    ("conv4s2", 2, 64, 128, 32, 64, True), ("convT4s2", 2, 128, 64, 16, 16, True),
+    ("conv3r", 3, 128, 128, 32, 32, True), ("conv4s1", 2, 128, 256, 64, 64, True),
+    ("conv4s2", 3, 128, 192, 16, 16, False),
+    ("conv4s2", 2, 36, 36, 64, 64, False),   # n_valid % 16 != 0
+    ("conv4s2", 2, 55, 64, 64, 64, True)]))
+def test_fused_instance_norm_statistics(kind, n, cin, cout, h, w, fused, nsplit):
     """InstanceNorm statistics accumulated by the GEMM epilogue (sn_tap_gemm_desc.stats + sn_stats_finalize) equal the
     per-(image, channel) mean and 1/sqrt(biased variance + eps) of the conv output; planes smaller than a tile (several
     images per tile) are refused by the plan and fall back to sn_plane_stats."""
     from swapnet_b200 import ops
 
-    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, 3)
+    layer, x, wt, bias = make_layer(kind, n, cin, cout, h, w, nsplit)
     oh, ow = L.out_hw(kind, h, w)
     y = torch.zeros(n, oh, ow, cout, device=dev())
     stats = torch.zeros(n, cout, 2, dtype=torch.float64, device=dev())
@@ -727,10 +880,16 @@ def test_fused_instance_norm_statistics(kind, n, cin, cout, h, w, fused):
         ops.plane_stats(y, cout, stats)
     torch.cuda.synchronize()
     ref = ref_forward(kind, x.double(), wt.double(), bias.double())
+    sep = ""
+    if nsplit == 1:   # the statistics of the single-pass output: those of the operand model's
+        model = model_forward(layer)
+        _, s_ = check_single_pass(f"{kind} fwd", y, model, nhwc(ref), 1.5e-5, SP_SEP_FP16)
+        ref, sep = model.permute(0, 3, 1, 2).cpu(), f" (model vs exact {s_:.3e})"
     mean = ref.mean((2, 3))
     rstd = (ref.var((2, 3), unbiased=False) + 1e-5).rsqrt()
     e_m = ((stats[..., 0].cpu() - mean).abs().max() / ref.abs().max()).item()
     e_r = relmax(stats[..., 1].cpu(), rstd)
-    record(f"fused_in_stats[{kind},{n},{cin},{cout},{h}x{w}]", f"fused={layer.fused_stats} mean {e_m:.3e} rstd {e_r:.3e}")
+    tag = f"fused_in_stats[{kind},{n},{cin},{cout},{h}x{w}" + ("]" if nsplit == 3 else ",nsplit=1]")
+    record(tag, f"fused={layer.fused_stats} mean {e_m:.3e} rstd {e_r:.3e}{sep}")
     assert e_m < 1e-5 and e_r < 1e-5, (e_m, e_r)
     assert relmax(y.cpu(), nhwc(ref)) < 1.5e-5
