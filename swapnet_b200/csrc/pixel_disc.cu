@@ -11,8 +11,8 @@
 // bf16-split and unscaled; nsplit = 1 keeps the hi x hi product only.  One warp owns 16 pixels; the C fragment of one
 // GEMM is the A fragment of the next, so z1 -> z2 and dz2 -> dA1 -> dx never leave registers.  The weight gradients
 // dW2 = dz2^T a1 and dW1 = g1^T x contract over pixels: the block stages its 64-pixel tile transposed in shared memory
-// and accumulates both in registers across all its tiles; a constant-one row appended to a1 and x gives db2 and db1 from
-// the same MMAs.
+// and accumulates both in registers across all its tiles, each tile's partial promoted with round-to-nearest adds; a
+// constant-one row appended to a1 and x gives db2 and db1 from the same MMAs.
 //
 // Cross-block sums (statistics, weight gradients) use atomics, or per-block slots added in block order by
 // det_sum_slots (deterministic mode).  Blocks take contiguous tile ranges of a grid fixed by the shapes alone.
@@ -481,35 +481,32 @@ __global__ void __launch_bounds__(kThreads, 1) pixel_kernel(const Args a) {
         Xl[lane * 2 * kSP + 16 * warp + r] = in ? xbl[p * d.x_pitch + lane] : (uint16_t)0;
       }
       __syncthreads();
-      // dW2 (+ db2) += dz2^T [a1; 1]   and   dW1 (+ db1) += g1^T [x; 1]   over the tile's 64 pixels
+      // dW2 (+ db2) += dz2^T [a1; 1]   and   dW1 (+ db1) += g1^T [x; 1]   over the tile's 64 pixels.  Each output
+      // fragment's 64-pixel partial runs in a fresh MMA accumulator (the tensor cores' adds truncate) and is then
+      // promoted into the block's sums with round-to-nearest adds, so the error stays flat over the hundreds of tiles a
+      // block sums at training shapes.
+      auto tile_partial = [&](float (&acc)[4], int a_h, int a_l, int r, int b_h, int b_l, int nt) {
+        float p[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-      for (int kc = 0; kc < kTile / 16; ++kc) {
-#pragma unroll
-        for (int m = 0; m < 2; ++m) {
-          uint32_t ahf[4], alf[4];
-          const int row = (32 * warp + 16 * m + g) * kSP + 8 * kc + t;
-          ahf[0] = sm[oDzh + row]; ahf[1] = sm[oDzh + row + 8 * kSP];
-          ahf[2] = sm[oDzh + row + 4]; ahf[3] = sm[oDzh + row + 8 * kSP + 4];
-          alf[0] = sm[oDzl + row]; alf[1] = sm[oDzl + row + 8 * kSP];
-          alf[2] = sm[oDzl + row + 4]; alf[3] = sm[oDzl + row + 8 * kSP + 4];
-#pragma unroll
-          for (int nt = 0; nt < 9; ++nt) {
-            const int w = (8 * nt + g) * kSP + 8 * kc + t;
-            mma_split<true>(gw2[m][nt], ahf, alf, sm + oA1h + w, sm + oA1l + w, d.nsplit);
-          }
-        }
-        uint32_t ahf[4], alf[4];
-        const int row = (16 * warp + g) * kSP + 8 * kc + t;
-        ahf[0] = sm[oG1h + row]; ahf[1] = sm[oG1h + row + 8 * kSP];
-        ahf[2] = sm[oG1h + row + 4]; ahf[3] = sm[oG1h + row + 8 * kSP + 4];
-        alf[0] = sm[oG1l + row]; alf[1] = sm[oG1l + row + 8 * kSP];
-        alf[2] = sm[oG1l + row + 4]; alf[3] = sm[oG1l + row + 8 * kSP + 4];
-#pragma unroll
-        for (int nt = 0; nt < 5; ++nt) {
+        for (int kc = 0; kc < kTile / 16; ++kc) {
+          uint32_t ah[4], al[4];
+          const int row = r * kSP + 8 * kc + t;
+          ah[0] = sm[a_h + row]; ah[1] = sm[a_h + row + 8 * kSP];
+          ah[2] = sm[a_h + row + 4]; ah[3] = sm[a_h + row + 8 * kSP + 4];
+          al[0] = sm[a_l + row]; al[1] = sm[a_l + row + 8 * kSP];
+          al[2] = sm[a_l + row + 4]; al[3] = sm[a_l + row + 8 * kSP + 4];
           const int w = (8 * nt + g) * kSP + 8 * kc + t;
-          mma_split<true>(gw1[nt], ahf, alf, sm + oXh + w, sm + oXl + w, d.nsplit);
+          mma_split<true>(p, ah, al, sm + b_h + w, sm + b_l + w, d.nsplit);
         }
-      }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[i] = __fadd_rn(acc[i], p[i]);
+      };
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int nt = 0; nt < 9; ++nt) tile_partial(gw2[m][nt], oDzh, oDzl, 32 * warp + 16 * m + g, oA1h, oA1l, nt);
+#pragma unroll
+      for (int nt = 0; nt < 5; ++nt) tile_partial(gw1[nt], oG1h, oG1l, 16 * warp + g, oXh, oXl, nt);
       __syncthreads();   // the staging buffers are rewritten by the next tile
     }
   }
@@ -577,6 +574,9 @@ int check_desc(const sn_pixel_desc* d, const char* what) {
   SN_REQUIRE(d->n >= 1 && d->hw >= 1 && d->cin >= 1 && d->cin <= d->x_c && (d->x_c == 16 || d->x_c == KX) &&
                  d->x_pitch >= d->x_c && d->x_pitch % 2 == 0,
              "%s: cin %d, x_c %d (16 or 32), pitch %d", what, d->cin, d->x_c, d->x_pitch);
+  // x and its twin are read as 32-bit words (channel pairs): an odd channel offset would issue misaligned loads
+  SN_REQUIRE(((uintptr_t)d->x_hi | (uintptr_t)d->x_lo | (uintptr_t)d->xb_hi | (uintptr_t)d->xb_lo) % 4 == 0,
+             "%s: x and its bf16 twin must be 4-byte aligned (an even channel offset)", what);
   SN_REQUIRE(d->nsplit == 1 || d->nsplit == 3, "%s: nsplit must be 1 or 3", what);
   SN_REQUIRE(!d->norm || d->stats, "%s: instance norm needs the statistics buffer", what);
   SN_REQUIRE(!d->slots || d->slots_cap >= sn_pixel_det_slots(d->n, d->cin), "%s: %lld slots given, %lld needed", what,
@@ -652,10 +652,13 @@ int sn_pixel_bwd_apply(const sn_pixel_desc* d, void* stream) {
   if (d->norm) rc = wg ? launch<PASS_APPLY, true, true>(d, st) : launch<PASS_APPLY, true, false>(d, st);
   else rc = wg ? launch<PASS_APPLY, false, true>(d, st) : launch<PASS_APPLY, false, false>(d, st);
   if (rc) return rc;
-  if (d->slots && wg) {
+  if (d->slots) {
+    // the slots this pass wrote: dW1 / dW2 with the weight gradients, dw3 / db3 here only without instance norm (the
+    // reduce pass sums them otherwise), with or without dW1 / dW2
     const WgSlots S = wg_slots(d->slots, d->n, d->cin);
     struct { const float* s; long long count; float* dst; } sums[] = {
-        {S.dw2, C2 * C1, d->dw2}, {S.db2, C2, d->db2}, {S.dw1, (long long)C1 * d->cin, d->dw1}, {S.db1, C1, d->db1},
+        {S.dw2, C2 * C1, wg ? d->dw2 : nullptr}, {S.db2, C2, wg ? d->db2 : nullptr},
+        {S.dw1, (long long)C1 * d->cin, wg ? d->dw1 : nullptr}, {S.db1, C1, wg ? d->db1 : nullptr},
         {S.dw3, C2, d->norm ? nullptr : d->dw3}, {S.db3, 1, d->norm ? nullptr : d->db3}};
     for (auto& s : sums) {
       if (!s.dst) continue;

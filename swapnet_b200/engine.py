@@ -527,10 +527,15 @@ class PixelGANEngine(Engine):
             raise NotImplementedError("--discriminator pixel --norm batch: batch statistics couple the samples inside "
                                       "the fused per-pixel passes, which normalise per image; use --norm instance or "
                                       "none")
+        if net.input_nc > M.PIXEL_MAX_INPUT_NC:
+            raise ValueError(f"PixelGANEngine: {net.input_nc} input channels; the fused per-pixel passes take at most "
+                             f"{M.PIXEL_MAX_INPUT_NC}")
         B, S, dev = batch, size, self.device
         self.batch, self.size = B, S
         self.din = din if din is not None else self.planes(B, S, S, L.padc(net.input_nc))
-        assert (self.din.n, self.din.h, self.din.w) == (B, S, S) and self.din.c in (16, 32)
+        if (self.din.n, self.din.h, self.din.w) != (B, S, S) or self.din.c not in (16, 32):
+            raise ValueError(f"PixelGANEngine: operand [{self.din.n}, {self.din.h}, {self.din.w}, {self.din.c}] for "
+                             f"batch {B} at {S}x{S}; the passes read 16 or 32 channels")
         self.pred = torch.zeros(B, S, S, device=dev)
         norm = net.norm == "instance"
         self.stats = torch.zeros(B, 128, 2, dtype=torch.float64, device=dev) if norm else None

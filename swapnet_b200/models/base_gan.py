@@ -21,7 +21,8 @@ What runs differently from the eager reference (results unchanged):
 Unsupported option values raise (there is no eager fallback): --gan_mode wgan-gp / dragan-gp / dragan-lp (the
 gradient penalty needs a second derivative through D), --gan_mode mescheder-r1-gp / mescheder-r2-gp (the reference's
 GANLoss raises for them too), --gan_label_mode hard (crashes in the reference too), --discriminator pixel with
---norm batch (batch statistics would couple the samples inside its fused per-pixel passes).
+--norm batch (batch statistics would couple the samples inside its fused per-pixel passes) or on a discriminator input
+of more than 32 channels (pix2pix's 58: the passes are 32 channels wide).
 --norm batch under data parallelism needs --b200_sync_bn 1: every train-mode BatchNorm2d call then normalises with the
 statistics of all ranks' samples (parallel.BNStatsExchange), so that 2 ranks x B/2 samples still reproduce one process
 with the full batch B; without the flag it is refused, since per-rank statistics would quietly break that equivalence.
@@ -180,6 +181,10 @@ class BaseGAN(BaseModel, ABC):
                 raise NotImplementedError("--discriminator pixel --norm batch is not provided: batch statistics couple "
                                           "the samples inside the fused per-pixel passes (csrc/pixel_disc.cu), which "
                                           "normalise per image; use --norm instance or none")
+            if opt.discriminator == "pixel" and self.get_D_inchannels() > M.PIXEL_MAX_INPUT_NC:
+                raise NotImplementedError(f"--discriminator pixel takes at most {M.PIXEL_MAX_INPUT_NC} input channels "
+                                          f"(the width of the fused per-pixel passes, csrc/pixel_disc.cu); this model's "
+                                          f"discriminator reads {self.get_D_inchannels()}")
             self._bn_sync = batch_norm_exchange(opt, self._world, opt.norm == "batch" or any(
                 isinstance(m, torch.nn.BatchNorm2d) for m in self.net_generator.modules()))
             if opt.discriminator == "pixel":     # --n_layers_D is ignored, as in the reference

@@ -128,10 +128,14 @@ class NLayerDiscriminator(_NoEager):
                 for i in self.conv_index[:-1]] + [None]
 
 
+PIXEL_MAX_INPUT_NC = 32   # the widest operand the fused passes of csrc/pixel_disc.cu read (KX)
+
+
 class PixelDiscriminator(_NoEager):
     """The 1x1 PatchGAN ('pixel', discriminators.py:138-168): net.0 Conv 1x1 input_nc -> ndf (bias), net.1 LeakyReLU,
     net.2 Conv ndf -> 2 ndf, net.3 the norm slot, net.4 LeakyReLU, net.5 Conv 2 ndf -> 1.  As in the reference, net.2 and
-    net.5 have a bias only with InstanceNorm2d.  ndf = 64 only (csrc/pixel_disc.cu's widths)."""
+    net.5 have a bias only with InstanceNorm2d.  ndf = 64 and input_nc <= PIXEL_MAX_INPUT_NC only (csrc/pixel_disc.cu's
+    widths)."""
 
     def __init__(self, input_nc, ndf=64, norm="instance"):
         super().__init__()
