@@ -478,15 +478,6 @@ int sn_feat_loss_fwd_bwd(const float* y_out, int po, const float* y_tgt, int pt,
 int sn_feat_loss_fwd_bwd_det(const float* y_out, int po, const float* y_tgt, int pt, long long npix, int c,
                              double weight, double gscale, double* loss_acc, float* dx, int pdx, double* slots,
                              long long slots_cap, void* stream);
-/* gram_matrix (perceptual.py:6-10) of the rows r = (b, ch): X_r[p] = src[b*s_n + ch*s_c + p*s_p];
- * gram: double [n*c][n*c] (zeroed here).  n*c <= 96. */
-int sn_gram(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix, double* gram,
-            void* stream);
-/* deterministic variant: per-block partial Gram matrices in `slots` (sn_gram_det_slots(n*c) doubles are enough), added
- * in block order.  sn_gram_mse is one block and needs no variant. */
-int sn_gram_det(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
-                double* gram, double* slots, long long slots_cap, void* stream);
-long long sn_gram_det_slots(int rows);
 
 /* ------------------------------------------------------------------------------------------
  * 1x1 PixelGAN discriminator (discriminators.py:138-168, csrc/pixel_disc.cu): per pixel
@@ -525,14 +516,9 @@ int sn_pixel_bwd_reduce(const sn_pixel_desc* d, void* stream);
  * dw3/db3 */
 int sn_pixel_bwd_apply(const sn_pixel_desc* d, void* stream);
 long long sn_pixel_det_slots(int n, int cin);
-/* *loss_acc += weight * MSELoss(gram_out, gram_tgt);  m[r][j] = d(that)/d(gram_out) + transpose (fp32). */
-int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double weight, double* loss_acc, float* m,
-                void* stream);
-/* dx[b, p, ch] (+)= sum_j m[b*c + ch][j] X_j[p]  — the style-loss gradient w.r.t. the raw image; dx NHWC fp32. */
-int sn_gram_bwd(const float* m, const float* src, long long s_n, long long s_c, long long s_p, int n, int c,
-                long long npix, float* dx, int dx_pitch, int accumulate, void* stream);
-/* Row blocks of a Gram matrix of any size (the style term over every rank's samples, or over more than 96 rows):
- * out: double [n_a*c][n_b*c] (zeroed here) = A B^T, the rows of A read as in sn_gram from a (strides a_n, a_c, a_p; n_a
+/* The style term (perceptual.py:6-10,58-63) over row blocks of a Gram matrix of any size: the whole matrix of one
+ * GPU's samples (a = b), or one rank's rows against every rank's.  Row r = (s, ch) of a tensor reads
+ * X_r[p] = a[s*a_n + ch*a_c + p*a_p].  out: double [n_a*c][n_b*c] (zeroed here) = A B^T, the rows of A from a (n_a
  * samples), those of B from b (n_b >= n_a samples).  fp32 sums over each 128-pixel chunk, fp64 from there on. */
 int sn_gram_rows(const float* a, long long a_n, long long a_c, long long a_p, int n_a, const float* b, long long b_n,
                  long long b_c, long long b_p, int n_b, int c, long long npix, double* out, void* stream);
@@ -544,11 +530,12 @@ int sn_gram_rows_det(const float* a, long long a_n, long long a_c, long long a_p
 long long sn_gram_rows_det_slots(int rows_l, int rows);
 /* For a [rows_l][rows] row block of the Gram matrices: *loss_acc += weight * sum((gram_out - gram_tgt)^2) / rows^2
  * (this block's share of weight * MSELoss over the whole [rows][rows] matrices);  m = gscale * (d/d(gram_out) + transpose)
- * on those rows (fp32).  One block: deterministic.  rows_l = rows, gscale = 1 gives sn_gram_mse's bits. */
+ * on those rows (fp32).  One block: deterministic. */
 int sn_gram_rows_mse(const double* gram_out, const double* gram_tgt, int rows_l, int rows, double weight,
                      double gscale, double* loss_acc, float* m, void* stream);
 /* dx[b, p, ch] (+)= sum_j m[b*c + ch][j] X_j[p] for the rows_l rows of m (whole samples b < rows_l / c) and the n*c
- * rows X_j of src (strides as in sn_gram); dx NHWC fp32 [rows_l / c][npix][dx_pitch]. */
+ * rows X_j of src (strides as in sn_gram_rows); dx NHWC fp32 [rows_l / c][npix][dx_pitch]: the style-loss gradient
+ * w.r.t. the raw image. */
 int sn_gram_rows_bwd(const float* m, int rows_l, const float* src, long long s_n, long long s_c, long long s_p, int n,
                      int c, long long npix, float* dx, int dx_pitch, int accumulate, void* stream);
 

@@ -199,12 +199,7 @@ SIGNATURES = {
     "sn_relu_pool_fwd": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_relu_pool_bwd": (_I, [_VP, _I, _VP, _I, _VP, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _I, _VP]),
     "sn_feat_loss_fwd_bwd": (_I, [_VP, _I, _VP, _I, _LL, _I, C.c_double, C.c_double, _VP, _VP, _I, _VP]),
-    "sn_gram": (_I, [_VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP]),
-    "sn_gram_det": (_I, [_VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP, _LL, _VP]),
-    "sn_gram_det_slots": (_LL, [_I]),
     "sn_feat_loss_fwd_bwd_det": (_I, [_VP, _I, _VP, _I, _LL, _I, C.c_double, C.c_double, _VP, _VP, _I, _VP, _LL, _VP]),
-    "sn_gram_mse": (_I, [_VP, _VP, _I, C.c_double, _VP, _VP, _VP]),
-    "sn_gram_bwd": (_I, [_VP, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _I, _I, _VP]),
     "sn_gram_rows": (_I, [_VP, _LL, _LL, _LL, _I, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP]),
     "sn_gram_rows_det": (_I, [_VP, _LL, _LL, _LL, _I, _VP, _LL, _LL, _LL, _I, _I, _LL, _VP, _VP, _LL, _VP]),
     "sn_gram_rows_det_slots": (_LL, [_I, _I]),

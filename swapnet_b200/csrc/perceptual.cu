@@ -238,120 +238,14 @@ __global__ void __launch_bounds__(kThreads) feat_loss_kernel(const float* __rest
 }
 
 // ---------------------------------------------------------------------------------
-// Gram matrix of R = n*c rows of npix pixels: G[i][j] = sum_p X_i[p] X_j[p]
-// row r = (b, ch): X_r[p] = src[b*sn + ch*sc + p*sp]
+// The style term: row blocks of the Gram matrix of R = n*c rows of npix pixels, G[i][j] = sum_p X_i[p] X_j[p], row
+// r = (b, ch): X_r[p] = src[b*sn + ch*sc + p*sp].  out[i][j] = sum_p A_i[p] B_j[p] for the R_l rows of A and the R rows
+// of B: the whole matrix (A = B), or one rank's rows against every rank's.  Nothing is sized by the row count: the
+// output is cut into kRowT x kRowT tiles (blockIdx.x) and the pixel chunks are split over blockIdx.y.  Each 128-pixel
+// chunk is summed in fp32; the chunk sums are added in fp64, so an entry's fp32 chain is one chunk long whatever the
+// split.
 // ---------------------------------------------------------------------------------
-constexpr int kGramP = 128;       // pixels per smem tile
-constexpr int kGramMaxR = 96;
-constexpr int kGramAcc = (kGramMaxR * kGramMaxR + kThreads - 1) / kThreads;  // 36
-
-// DET: the block's partial Gram matrix goes to slots[blockIdx.x][R*R] (det_sum_slots adds the blocks in order)
-template <bool DET>
-__global__ void __launch_bounds__(kThreads) gram_kernel(const float* __restrict__ src, long long sn, long long sc,
-                                                         long long sp, int C, int R, long long npix,
-                                                         double* __restrict__ G, double* __restrict__ slots) {
-  extern __shared__ float tile[];   // [R][kGramP + 1]
-  constexpr int TP = kGramP + 1;
-  float acc[kGramAcc];
-#pragma unroll
-  for (int k = 0; k < kGramAcc; ++k) acc[k] = 0.f;
-  const long long nchunks = (npix + kGramP - 1) / kGramP;
-  for (long long ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
-    const long long p0 = ch * kGramP;
-    __syncthreads();
-    for (int i = threadIdx.x; i < R * kGramP; i += blockDim.x) {
-      int r, p;
-      if (sp == 1) { r = i / kGramP; p = i - r * kGramP; } else { p = i / R; r = i - p * R; }
-      const int b = r / C, c = r - b * C;
-      tile[r * TP + p] = (p0 + p < npix) ? src[b * sn + c * sc + (p0 + p) * sp] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < kGramAcc; ++k) {
-      const int idx = k * kThreads + threadIdx.x;
-      if (idx < R * R) {
-        const int i = idx / R, j = idx - i * R;
-        const float* a = tile + i * TP;
-        const float* b = tile + j * TP;
-        float s = 0.f;
-#pragma unroll 8
-        for (int p = 0; p < kGramP; ++p) s += a[p] * b[p];
-        acc[k] += s;
-      }
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < kGramAcc; ++k) {
-    const int idx = k * kThreads + threadIdx.x;
-    if (idx < R * R) {
-      if constexpr (DET) slots[(long long)blockIdx.x * R * R + idx] = (double)acc[k];
-      else atomicAdd(&G[idx], (double)acc[k]);
-    }
-  }
-}
-
-// loss_acc += weight * mean((Go - Gt)^2);  M = 4 * weight * (Go - Gt) / R^2  (= dL/dGo + its transpose)
-__global__ void gram_mse_kernel(const double* __restrict__ Go, const double* __restrict__ Gt, int R, double weight,
-                                double* __restrict__ loss_acc, float* __restrict__ M) {
-  __shared__ double red[kThreads];
-  double l = 0.0;
-  const double inv = 1.0 / ((double)R * R);
-  for (int i = threadIdx.x; i < R * R; i += blockDim.x) {
-    const double d = Go[i] - Gt[i];
-    l += d * d;
-    M[i] = (float)(4.0 * weight * d * inv);
-  }
-  red[threadIdx.x] = l;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) atomicAdd(loss_acc, weight * red[0] * inv);
-}
-
-// dx[b, p, ch] (+)= sum_j M[r][j] X_j[p], r = b*C + ch;  dx NHWC fp32 [n, npix, pitch]
-__global__ void __launch_bounds__(kThreads) gram_bwd_kernel(const float* __restrict__ M,
-                                                             const float* __restrict__ src, long long sn,
-                                                             long long sc, long long sp, int C, int R,
-                                                             long long npix, float* __restrict__ dx, int pdx,
-                                                             int accumulate) {
-  extern __shared__ float smem[];   // tile [R][kGramP + 1], then M [R][R]
-  constexpr int TP = kGramP + 1;
-  float* tile = smem;
-  float* Ms = smem + R * TP;
-  for (int i = threadIdx.x; i < R * R; i += blockDim.x) Ms[i] = M[i];
-  const long long nchunks = (npix + kGramP - 1) / kGramP;
-  for (long long ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
-    const long long p0 = ch * kGramP;
-    __syncthreads();
-    for (int i = threadIdx.x; i < R * kGramP; i += blockDim.x) {
-      int r, p;
-      if (sp == 1) { r = i / kGramP; p = i - r * kGramP; } else { p = i / R; r = i - p * R; }
-      const int b = r / C, c = r - b * C;
-      tile[r * TP + p] = (p0 + p < npix) ? src[b * sn + c * sc + (p0 + p) * sp] : 0.f;
-    }
-    __syncthreads();
-    const int p = threadIdx.x % kGramP;
-    if (p0 + p < npix) {
-      for (int r = threadIdx.x / kGramP; r < R; r += kThreads / kGramP) {
-        float s = 0.f;
-        for (int j = 0; j < R; ++j) s += Ms[r * R + j] * tile[j * TP + p];
-        const int b = r / C, c = r - b * C;
-        float* d = dx + ((long long)b * npix + p0 + p) * pdx + c;
-        *d = accumulate ? *d + s : s;
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------
-// Row blocks of a Gram matrix with any number of rows: the style term over every rank's samples, or over more than
-// kGramMaxR rows on one GPU.  out[i][j] = sum_p A_i[p] B_j[p] for the R_l rows of A and the R rows of B, each row
-// r = (b, ch) read as in gram_kernel.  Nothing is sized by the row count: the output is cut into kRowT x kRowT tiles
-// (blockIdx.x) and the pixel chunks are split over blockIdx.y.  Each 128-pixel chunk is summed in fp32 as in
-// gram_kernel; the chunk sums are added in fp64, so an entry's fp32 chain is one chunk long whatever the split.
-// ---------------------------------------------------------------------------------
+constexpr int kGramP = 128;                    // pixels per smem tile
 constexpr int kRowT = 32;                      // rows per tile edge
 constexpr int kRowBlocks = 4 * SN_NUM_SMS;     // target block count of gram_rows / gram_rows_bwd
 
@@ -422,8 +316,9 @@ __global__ void __launch_bounds__(kThreads) gram_rows_kernel(RowSrc a, RowSrc b,
 }
 
 // loss_acc += weight * sum((Go - Gt)^2) / R^2 over an [R_l][R] row block;  M = 4 * weight * gscale * (Go - Gt) / R^2
-// (= gscale * (dL/dGo + its transpose) on those rows, the Gram matrices being symmetric).  gram_mse_kernel's arithmetic:
-// with R_l = R and gscale = 1 both give the same bits.
+// (= gscale * (dL/dGo + its transpose) on those rows, the Gram matrices being symmetric).  One block, fp64 throughout:
+// each thread's strided squares, a tree over the threads, one atomicAdd.  M is rounded to fp32 once, from
+// (4 * weight * gscale * d) * (1 / R^2).
 __global__ void gram_rows_mse_kernel(const double* __restrict__ Go, const double* __restrict__ Gt, long long n, int R,
                                      double weight, double gscale, double* __restrict__ loss_acc,
                                      float* __restrict__ M) {
@@ -447,7 +342,7 @@ __global__ void gram_rows_mse_kernel(const double* __restrict__ Go, const double
 
 // dx[b, p, ch] (+)= sum_j M[r][j] X_j[p] for the R_l rows r = b*C + ch of M and the R rows of X.  Block (x, y): row
 // tile y (kRowT rows of M), pixel chunks x, x + gridDim.x, ...; thread t owns pixel t % 128 of rows t/128 + 2k.
-// The columns j are summed in order in fp32 (the zero rows past R add exact zeros), as in gram_bwd_kernel.
+// The columns j are summed in order in fp32 (the zero rows past R add exact zeros): one fp32 chain of R terms per entry.
 __global__ void __launch_bounds__(kThreads) gram_rows_bwd_kernel(const float* __restrict__ M, RowSrc x, int C, int Rl,
                                                                   int R, long long npix, float* __restrict__ dx,
                                                                   int pdx, int accumulate) {
@@ -589,78 +484,6 @@ int sn_feat_loss_fwd_bwd_det(const float* y_out, int po, const float* y_tgt, int
   SN_REQUIRE(slots, "feat_loss_det: null slots");
   return feat_loss_impl(y_out, po, y_tgt, pt, npix, c, weight, gscale, loss_acc, dx, pdx, slots, slots_cap,
                         (cudaStream_t)stream);
-}
-
-constexpr int kGramMaxBlocks = 296;
-
-static int gram_impl(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
-                     double* gram, double* slots, long long slots_cap, cudaStream_t st) {
-  SN_REQUIRE(src && gram, "null pointer");
-  const int R = n * c;
-  SN_REQUIRE(R >= 1 && R <= kGramMaxR, "gram: n*c = %d rows, at most %d supported", R, kGramMaxR);
-  SN_CHECK_CUDA(cudaMemsetAsync(gram, 0, sizeof(double) * R * R, st));
-  const size_t smem = (size_t)R * (kGramP + 1) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr = true;
-  }
-  long long chunks = (npix + kGramP - 1) / kGramP;
-  const int grid = (int)(chunks < kGramMaxBlocks ? chunks : kGramMaxBlocks);
-  if (!slots) {
-    gram_kernel<false><<<grid, kThreads, smem, st>>>(src, s_n, s_c, s_p, c, R, npix, gram, nullptr);
-    LAUNCH_CHECK();
-    return SN_OK;
-  }
-  SN_REQUIRE((long long)grid * R * R <= slots_cap, "gram_det: %lld slots needed, %lld given", (long long)grid * R * R,
-             slots_cap);
-  gram_kernel<true><<<grid, kThreads, smem, st>>>(src, s_n, s_c, s_p, c, R, npix, gram, slots);
-  LAUNCH_CHECK();
-  SN_CHECK_CUDA(det_sum_slots(slots, grid, (long long)R * R, gram, st));
-  LAUNCH_CHECK();
-  return SN_OK;
-}
-
-int sn_gram(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix, double* gram,
-            void* stream) {
-  return gram_impl(src, s_n, s_c, s_p, n, c, npix, gram, nullptr, 0, (cudaStream_t)stream);
-}
-
-int sn_gram_det(const float* src, long long s_n, long long s_c, long long s_p, int n, int c, long long npix,
-                double* gram, double* slots, long long slots_cap, void* stream) {
-  SN_REQUIRE(slots, "gram_det: null slots");
-  return gram_impl(src, s_n, s_c, s_p, n, c, npix, gram, slots, slots_cap, (cudaStream_t)stream);
-}
-
-long long sn_gram_det_slots(int rows) { return (long long)kGramMaxBlocks * rows * rows; }
-
-int sn_gram_mse(const double* gram_out, const double* gram_tgt, int rows, double weight, double* loss_acc, float* m,
-                void* stream) {
-  SN_REQUIRE(gram_out && gram_tgt && loss_acc && m, "null pointer");
-  gram_mse_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(gram_out, gram_tgt, rows, weight, loss_acc, m);
-  LAUNCH_CHECK();
-  return SN_OK;
-}
-
-int sn_gram_bwd(const float* m, const float* src, long long s_n, long long s_c, long long s_p, int n, int c,
-                long long npix, float* dx, int dx_pitch, int accumulate, void* stream) {
-  SN_REQUIRE(m && src && dx, "null pointer");
-  const int R = n * c;
-  SN_REQUIRE(R >= 1 && R <= kGramMaxR, "gram_bwd: n*c = %d rows, at most %d supported", R, kGramMaxR);
-  cudaStream_t st = (cudaStream_t)stream;
-  static bool attr = false;
-  if (!attr) {
-    SN_CHECK_CUDA(cudaFuncSetAttribute(gram_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr = true;
-  }
-  const size_t smem = ((size_t)R * (kGramP + 1) + (size_t)R * R) * sizeof(float);
-  long long chunks = (npix + kGramP - 1) / kGramP;
-  const int grid = (int)(chunks < 592 ? chunks : 592);
-  gram_bwd_kernel<<<grid, kThreads, smem, st>>>(m, src, s_n, s_c, s_p, c, R, npix, dx, dx_pitch, accumulate);
-  LAUNCH_CHECK();
-  return SN_OK;
 }
 
 // pixel splits of gram_rows: enough blocks for kRowBlocks whatever the tile count, at most one per chunk

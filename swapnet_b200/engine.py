@@ -801,12 +801,10 @@ class PerceptualEngine:
     content = sum over 5 taps of MSE(f_out, f_tgt), f = L2-normalised ReLU features of `2x - 1`;
     style   = 5 * MSE(gram(out), gram(tgt)) of the raw images viewed as [B*3, H*W] (perceptual.py:58-63).
 
-    The style term has two device paths.  Up to 96 rows on one rank, `gram` / `gram_mse` / `gram_bwd` hold the whole
-    Gram matrix in one block's registers and shared memory.  Beyond that, or with a style exchange (`--b200_sync_style 1`
-    under data parallelism), the row kernels compute this rank's [R_l, R] row block of a Gram matrix of any size.
+    The style term runs on the row kernels (`gram_rows`, `gram_rows_mse`, `gram_rows_bwd`), which compute this rank's
+    [R_l, R] row block of a Gram matrix of any size: the whole matrix of this rank's samples (R_l = R), or with a style
+    exchange (`--b200_sync_style 1` under data parallelism) this rank's rows against every rank's.
     """
-
-    KGRAM_MAX_ROWS = 96     # csrc/perceptual.cu kGramMaxR: the most rows `gram` / `gram_bwd` accept
 
     def __init__(self, net: Optional[M.VGG16Features], batch: int, size: int, device, nsplit: int = 3,
                  content: bool = True, deterministic: bool = False, style_exchange=None):
@@ -829,7 +827,6 @@ class PerceptualEngine:
         rl = 3 * batch
         r = rl * world
         self.rows_l, self.rows = rl, r
-        self.row_path = ex is not None or r > self.KGRAM_MAX_ROWS
         self.gram_o = torch.zeros(rl, r, dtype=torch.float64, device=dev)
         self.gram_t = torch.zeros(rl, r, dtype=torch.float64, device=dev)
         self.gram_m = torch.zeros(rl, r, dtype=torch.float32, device=dev)
@@ -876,28 +873,18 @@ class PerceptualEngine:
         With a style exchange: the Gram matrices of every rank's samples; acc receives the full-batch loss (the same
         bits on every rank) and grad_accum `world` times the full-batch gradient w.r.t. this rank's fakes."""
         ex = self.style_exchange
-        if not self.row_path:
-            ops.gram(fakes, True, self.gram_o, ws=self.det_ws)
-            ops.gram(targets, False, self.gram_t, ws=self.det_ws)
-            ops.gram_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
-            ops.gram_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)
-            return
-        if ex is None:       # one rank, more rows than `gram` holds: the whole matrix as one row block
-            ops.gram_rows(fakes, fakes, True, self.gram_o, ws=self.det_ws)
-            ops.gram_rows(targets, targets, False, self.gram_t, ws=self.det_ws)
-            ops.gram_rows_mse(self.gram_o, self.gram_t, 5.0 * lam, acc, self.gram_m)
-            ops.gram_rows_bwd(self.gram_m, fakes, True, grad_accum, accumulate=True)
-            return
-        fa = ex.gather(fakes, self.fakes_all)
-        ta = ex.gather(targets, self.targets_all)
+        fa, ta, part, world = fakes, targets, acc, 1
+        if ex is not None:
+            fa, ta = ex.gather(fakes, self.fakes_all), ex.gather(targets, self.targets_all)
+            part, world = self.style_part.zero_(), ex.world
         ops.gram_rows(fakes, fa, True, self.gram_o, ws=self.det_ws)       # rows of this rank x rows of all ranks
         ops.gram_rows(targets, ta, False, self.gram_t, ws=self.det_ws)
-        self.style_part.zero_()
         # m is scaled by `world`: the optimizer multiplies the summed G gradients by 1/world (BaseGAN.grad_scale),
         # because every other term is a mean over the rank's shard and so world times its share of the full-batch
         # gradient.  m @ X_all already is the full-batch gradient w.r.t. this rank's fakes, not a shard mean.
-        ops.gram_rows_mse(self.gram_o, self.gram_t, 5.0 * lam, self.style_part, self.gram_m, gscale=float(ex.world))
+        ops.gram_rows_mse(self.gram_o, self.gram_t, 5.0 * lam, part, self.gram_m, gscale=float(world))
         ops.gram_rows_bwd(self.gram_m, fa, True, grad_accum, accumulate=True)
-        parts = ex.gather(self.style_part, self.style_parts)
-        for r in range(ex.world):         # rank order, on every rank: every rank reports the same bits
-            acc.add_(parts[r:r + 1])
+        if ex is not None:
+            parts = ex.gather(self.style_part, self.style_parts)
+            for r in range(ex.world):         # rank order, on every rank: every rank reports the same bits
+                acc.add_(parts[r:r + 1])

@@ -1024,37 +1024,11 @@ def _gram_strides(x: torch.Tensor, nhwc: bool):
     return n, c, h * w, c * h * w, h * w, 1
 
 
-def gram(x: torch.Tensor, nhwc: bool, out: torch.Tensor, ws: Optional[DetWorkspace] = None) -> None:
-    """out [n*c, n*c] (float64) = gram_matrix(x) of perceptual.py:6-10 (rows = (sample, channel))."""
-    n, c, npix, sn, sc, sp = _gram_strides(x, nhwc)
-    assert out.dtype == torch.float64 and out.numel() == (n * c) ** 2
-    if ws is not None:
-        sl = ws.get(int(_lib.load().sn_gram_det_slots(n * c)))
-        check(_lib.load().sn_gram_det(x.data_ptr(), sn, sc, sp, n, c, npix, out.data_ptr(), sl.data_ptr(), sl.numel(),
-                                      _stream()))
-        return
-    check(_lib.load().sn_gram(x.data_ptr(), sn, sc, sp, n, c, npix, out.data_ptr(), _stream()))
-
-
-def gram_mse(g_out: torch.Tensor, g_tgt: torch.Tensor, weight: float, loss_acc: torch.Tensor, m: torch.Tensor) -> None:
-    rows = g_out.shape[0]
-    assert m.dtype == torch.float32 and m.numel() == rows * rows
-    check(_lib.load().sn_gram_mse(g_out.data_ptr(), g_tgt.data_ptr(), rows, weight, loss_acc.data_ptr(), m.data_ptr(),
-                                  _stream()))
-
-
-def gram_bwd(m: torch.Tensor, x: torch.Tensor, nhwc: bool, dx: torch.Tensor, accumulate: bool) -> None:
-    """dx (NHWC fp32 [n,h,w,>=c]) (+)= m @ X."""
-    n, c, npix, sn, sc, sp = _gram_strides(x, nhwc)
-    assert dx.shape[0] == n and dx.shape[1] * dx.shape[2] == npix
-    check(_lib.load().sn_gram_bwd(m.data_ptr(), x.data_ptr(), sn, sc, sp, n, c, npix, dx.data_ptr(), _pitch(dx),
-                                  1 if accumulate else 0, _stream()))
-
-
 def gram_rows(a: torch.Tensor, b: torch.Tensor, nhwc: bool, out: torch.Tensor,
               ws: Optional[DetWorkspace] = None) -> None:
     """out [n_a*c, n_b*c] (float64) = A B^T: the rows (sample, channel) of `a` against those of `b` (same layout and
-    image size; b may hold more samples, e.g. every rank's).  Any number of rows."""
+    image size; b may hold more samples, e.g. every rank's).  With a = b: gram_matrix(a) of perceptual.py:6-10.  Any
+    number of rows."""
     na, c, npix, an, ac, ap = _gram_strides(a, nhwc)
     nb, cb, npix_b, bn, bc, bp = _gram_strides(b, nhwc)
     assert (cb, npix_b) == (c, npix) and out.dtype == torch.float64 and out.shape == (na * c, nb * c)

@@ -358,9 +358,10 @@ def test_wgrad_plan_repeats_bit_identically(kind, cin, cout, hw, n, nsplit):
         assert ks >= 8
 
 
-def test_elementwise_reductions_repeat_bit_identically():
-    """plane statistics, the norm backward reduction, both bias-gradient kernels, the loss sums and the one-channel
-    logits' weight gradient: repeated launches with a workspace give the same bits, close to the atomic versions."""
+def test_reductions_repeat_bit_identically():
+    """plane statistics, the norm backward reduction, both bias-gradient kernels, the loss sums, the one-channel
+    logits' weight gradient and the style term's Gram rows: repeated launches with a workspace give the same bits, close
+    to the atomic versions."""
     from swapnet_b200 import ops
 
     g = torch.Generator().manual_seed(11)
@@ -432,8 +433,8 @@ def test_elementwise_reductions_repeat_bit_identically():
     for img, nhwc in ((torch.randn(8, 256, 256, 3, generator=g), True), (torch.randn(8, 3, 256, 256, generator=g), False)):
         img = img.to(dev())
         gm = torch.zeros(24, 24, dtype=torch.float64, device=dev())
-        a = _repeat(lambda: ops.gram(img, nhwc, gm, ws=ws), gm)
-        assert relmax(a, _repeat(lambda: ops.gram(img, nhwc, gm), gm, 1)) < 1e-9
+        a = _repeat(lambda: ops.gram_rows(img, img, nhwc, gm, ws=ws), gm)
+        assert relmax(a, _repeat(lambda: ops.gram_rows(img, img, nhwc, gm), gm, 1)) < 1e-9
         x64 = (img.permute(0, 3, 1, 2) if nhwc else img).reshape(24, -1).double()
         assert relmax(a, x64 @ x64.T) < 1e-6
     record("det_slot_workspace_bytes[kernel tests]", ws.nbytes)

@@ -760,7 +760,7 @@ def test_feat_loss(c):
 
 
 @pytest.mark.parametrize("n,s", [(2, 32), (16, 64), (1, 48)])
-def test_gram_style_loss(n, s):
+def test_gram_rows_style_loss(n, s):
     """5 x MSE(gram(out), gram(tgt)) on raw images viewed as [B*3, H*W] (perceptual.py:6-10,58-63)"""
     from swapnet_b200 import ops
 
@@ -781,18 +781,19 @@ def test_gram_style_loss(n, s):
     gt = torch.zeros_like(go)
     m = torch.zeros(r, r, device=dev())
     fk = nhwc(out).to(dev())
-    ops.gram(fk, True, go)
-    ops.gram(tgt.to(dev()), False, gt)
+    tg = tgt.to(dev())
+    ops.gram_rows(fk, fk, True, go)
+    ops.gram_rows(tg, tg, False, gt)
     assert relmax(go.cpu(), gram(out.double())) < 1e-5 and relmax(gt.cpu(), gram(tgt.double())) < 1e-5
     acc = torch.zeros(1, dtype=torch.float64, device=dev())
-    ops.gram_mse(go, gt, 5 * lam, acc, m)
+    ops.gram_rows_mse(go, gt, 5 * lam, acc, m)
     assert abs(acc.item() - loss.item()) < 1e-4 * abs(loss.item())
     dx = torch.full((n, s, s, 3), 7.0, device=dev())
-    ops.gram_bwd(m, fk, True, dx, accumulate=False)
+    ops.gram_rows_bwd(m, fk, True, dx, accumulate=False)
     assert relmax(dx.cpu(), nhwc(gx)) < 1e-4
     base = torch.randn(n, s, s, 3, generator=g) * gx.abs().max().float()   # same magnitude as the L1 gradient it joins
     dx = base.clone().to(dev())
-    ops.gram_bwd(m, fk, True, dx, accumulate=True)
+    ops.gram_rows_bwd(m, fk, True, dx, accumulate=True)
     assert relmax(dx.cpu(), base.double() + nhwc(gx)) < 1e-4
 
 

@@ -3,11 +3,11 @@ fp64 torch of the same operation, at the training shapes and at the edges where 
 
 - affine_pack, relu_pool_fwd/bwd: exact operations (one fp32 multiply and add; a max; one fp32 add).  Their words must
   be common.cuh's split16 of the restated fp32 value, bit for bit.
-- feat_loss, gram, gram_mse, gram_bwd, to_one_fwd, tap_sum_fwd, to_one_wgrad, to_one_dgrad: fp32 sums.  Each entry's
-  error is normalised by the sum of the absolute values of its terms (for the Gram matrix by sqrt(G_ii G_jj), which
-  bounds that sum) and must stay under k u, u = 2^-24, with k the length of the longest chain of fp32 roundings that
-  forms the entry: the kernel's per-thread chain, its tree or row reduction, and its block sums.  These are worst-case
-  bounds; the measured values (in units of u) go to the parity log.
+- feat_loss, the style term (gram_rows, gram_rows_mse, gram_rows_bwd), to_one_fwd, tap_sum_fwd, to_one_wgrad,
+  to_one_dgrad: fp32 sums.  Each entry's error is normalised by the sum of the absolute values of its terms (for the
+  Gram matrix by sqrt(G_ii G_jj), which bounds that sum) and must stay under k u, u = 2^-24, with k the length of the
+  longest chain of fp32 roundings that forms the entry: the kernel's per-thread chain, its tree or row reduction, and
+  its block sums.  These are worst-case bounds; the measured values (in units of u) go to the parity log.
 - Operands that arrive as split planes are decoded first (dense_of): the fp64 reference is computed from the values the
   kernel reads, so the bounds measure the kernel's arithmetic, not the 16-bit encoding.
 - Every output is prefilled with a sentinel (NaN for fp32, SENT16 for plane words): each valid entry must be written,
@@ -293,7 +293,8 @@ def test_feat_loss_refusals():
 
 
 # ---- Gram matrix and the style term ----------------------------------------------------------------------------
-GRAM_P, GRAM_BLOCKS, GRAM_BWD_BLOCKS = 128, 296, 592
+GRAM_P = 128
+GRAM_K = GRAM_P + 2     # fp32 chain of one Gram entry: the 128 products of a chunk; the chunk sums are fp64
 
 
 def gram_source(n, c, npix, src_nhwc, g, lo=-1.0, hi=1.0):
@@ -305,122 +306,13 @@ def gram_source(n, c, npix, src_nhwc, g, lo=-1.0, hi=1.0):
     return x.view(n, c, 1, npix), rows
 
 
-def gram_k(npix):
-    """fp32 chain of one Gram entry: 128 products per chunk, then the block's chunks; the block sums are fp64."""
-    chunks = (npix + GRAM_P - 1) // GRAM_P
-    return GRAM_P + math.ceil(chunks / min(chunks, GRAM_BLOCKS)) + 2
-
-
 def gram_scale(gm):
     dg = gm.diagonal().abs()
     return torch.sqrt(dg[:, None] * dg[None, :])
 
 
-def run_gram(n, c, npix, src_nhwc, seed):
-    g = gen(seed)
-    x, rows = gram_source(n, c, npix, src_nhwc, g)
-    r = n * c
-    ref = rows @ rows.T
-    scale = gram_scale(ref)
-    ws = ops.DetWorkspace(dev())
-    outs = []
-    for det in (False, True, True):
-        out = torch.full((r, r), NAN, dtype=torch.float64, device=dev())   # the kernel must overwrite it
-        ops.gram(x, src_nhwc, out, ws=ws if det else None)
-        torch.cuda.synchronize()
-        bounded(f"gram[R={r},npix={npix},{'nhwc' if src_nhwc else 'nchw'},{'det' if det else 'atomic'}]", out, ref,
-                scale, gram_k(npix))
-        outs.append(out)
-    assert torch.equal(outs[1], outs[2]), "gram_det did not repeat bit for bit"
-
-
-@pytest.mark.parametrize("src_nhwc", [True, False])
-@pytest.mark.parametrize("npix", [1, 127, 128, 129, 128 * 296 - 1, 128 * 296 + 1])
-@pytest.mark.parametrize("n", [1, 16, 32])          # R = 3, 48, 96 (the largest the engine accepts)
-def test_gram(n, npix, src_nhwc):
-    run_gram(n, 3, npix, src_nhwc, seed=n * 7 + npix)
-
-
-@pytest.mark.parametrize("src_nhwc", [True, False])
-def test_gram_512(src_nhwc):
-    """The style term's shape at 512 x 512, batch 16: 48 rows of 2^18 pixels, 7 chunks per block in fp32."""
-    run_gram(16, 3, 512 * 512, src_nhwc, seed=512)
-
-
-def test_gram_refusals():
-    x = torch.zeros(1, 97, 2, 2, device=dev())                    # 97 rows from an NCHW source
-    refused(lambda: ops.gram(x, False, torch.zeros(97, 97, dtype=torch.float64, device=dev())))
-    refused(lambda: ops.gram_bwd(torch.zeros(97, 97, device=dev()), x, False, torch.zeros(1, 2, 2, 97, device=dev()),
-                                 accumulate=False))
-    x = torch.rand(16, 3, 1, 1000, device=dev())
-    grid = min((1000 + GRAM_P - 1) // GRAM_P, GRAM_BLOCKS)
-    gm = torch.zeros(48, 48, dtype=torch.float64, device=dev())
-    slots = torch.zeros(grid * 48 * 48, dtype=torch.float64, device=dev())
-
-    def call(cap):
-        _lib.check(_lib.load().sn_gram_det(x.data_ptr(), 3000, 1000, 1, 16, 3, 1000, gm.data_ptr(), slots.data_ptr(),
-                                           cap, _stream()))
-    refused(lambda: call(grid * 48 * 48 - 1))
-    call(grid * 48 * 48)
-    torch.cuda.synchronize()
-    rows = x.reshape(48, 1000).double()
-    bounded("gram_det[exact slot capacity]", gm, rows @ rows.T, gram_scale(rows @ rows.T), gram_k(1000))
-
-
-@pytest.mark.parametrize("r", [3, 48, 96])
-def test_gram_mse(r):
-    """One block of 256 threads: R = 96 takes 36 strides.  M = 4 w (Go - Gt) / R^2, restated in the kernel's order."""
-    g = gen(r)
-    go = torch.randn(r, r, generator=g, device=dev(), dtype=torch.float64) * 1e4
-    gt = torch.randn(r, r, generator=g, device=dev(), dtype=torch.float64) * 1e4
-    w, acc0 = 5.0 * 3e-8, 0.625
-    acc = torch.full((1,), acc0, dtype=torch.float64, device=dev())
-    m = torch.full((r, r), NAN, device=dev())
-    ops.gram_mse(go, gt, w, acc, m)
-    torch.cuda.synchronize()
-    d = go - gt
-    inv = 1.0 / (r * r)
-    assert torch.equal(m, (((4.0 * w) * d) * inv).float()), "M differs from fp32(4 w (Go - Gt) / R^2)"
-    loss = w * (d * d).sum().item() * inv
-    err = abs(acc.item() - acc0 - loss) / (acc0 + loss)
-    record(f"gram_mse[R={r}]", f"{err:.2e}")
-    assert err < 1e-14, err            # fp64 sums of R^2 positive terms
-
-
-GRAM_BWD_CASES = [(1, 1, True), (16, 129, False), (32, 127, True), (32, 128 * 592 + 1, False),
-                  (16, 128 * 592 + 1, True)]
-
-
-@pytest.mark.parametrize("n,npix,src_nhwc", GRAM_BWD_CASES)
-def test_gram_bwd(n, npix, src_nhwc):
-    """dx[b, p, ch] (+)= sum_j M[r][j] X_j[p] into a pitch-4 dx whose channel 3 holds a sentinel; 592 blocks stride
-    over the chunks from 128 * 592 + 1 pixels on."""
-    g = gen(n + npix)
-    x, rows = gram_source(n, 3, npix, src_nhwc, g)
-    r = 3 * n
-    m = torch.randn(r, r, generator=g, device=dev()) * 1e-3
-    prod = m.double() @ rows
-    mag = m.double().abs() @ rows.abs()
-
-    def as_dx(t):           # [R, npix] -> NHWC [n, 1, npix, 3]
-        return t.view(n, 3, npix).permute(0, 2, 1).reshape(n, 1, npix, 3)
-
-    base = torch.randn(n, 1, npix, 3, generator=g, device=dev()) * prod.abs().max().float()
-    for accumulate in (False, True):
-        dx = torch.full((n, 1, npix, 4), NAN, device=dev())
-        if accumulate:
-            dx[..., :3] = base
-        ops.gram_bwd(m, x, src_nhwc, dx, accumulate=accumulate)
-        torch.cuda.synchronize()
-        want = as_dx(prod) + (base.double() if accumulate else 0.0)
-        scale = as_dx(mag) + (base.double().abs() if accumulate else 0.0)
-        bounded(f"gram_bwd[R={r},npix={npix},{'nhwc' if src_nhwc else 'nchw'},accumulate={accumulate}]", dx[..., :3],
-                want, scale, r + 2)
-        assert bool(torch.isnan(dx[..., 3]).all()), "wrote channel 3"
-
-
 @pytest.mark.parametrize("det", [False, True])
-def test_style_term_training_shape(det):
+def test_gram_rows_style_term_training_shape(det):
     """PerceptualEngine.style at B = 16, S = 512 (R = 48) against fp64 autograd of 5 MSE(X X^T, T T^T) lambda."""
     B, S, lam = 16, 512, 1e-8
     g = gen(16 + det)
@@ -441,14 +333,13 @@ def test_style_term_training_shape(det):
     grad = gx.detach().view(B, 3, S, S).permute(0, 2, 3, 1)
     base = torch.randn(B, S, S, 3, generator=g, device=dev()) * grad.abs().max().float()   # the L1 gradient it joins
     dx = base.clone()
-    ops.gram(fakes, True, go, ws=ws)
-    ops.gram(targets, False, gt, ws=ws)
-    ops.gram_mse(go, gt, 5.0 * lam, acc, m)
-    ops.gram_bwd(m, fakes, True, dx, accumulate=True)
+    ops.gram_rows(fakes, fakes, True, go, ws=ws)
+    ops.gram_rows(targets, targets, False, gt, ws=ws)
+    ops.gram_rows_mse(go, gt, 5.0 * lam, acc, m)
+    ops.gram_rows_bwd(m, fakes, True, dx, accumulate=True)
     torch.cuda.synchronize()
     with torch.no_grad():
-        k = gram_k(npix)
-        dg = k * U * (gram_scale(go_ref) + gram_scale(gt_ref))            # |Go error| + |Gt error|, per entry
+        dg = GRAM_K * U * (gram_scale(go_ref) + gram_scale(gt_ref))            # |Go error| + |Gt error|, per entry
         d = (go_ref - gt_ref).abs()
         loss_bound = 5 * lam / r ** 2 * (2 * d * dg + dg * dg).sum().item()
         m_ref = 4 * 5 * lam * (go_ref - gt_ref) / r ** 2

@@ -1,14 +1,13 @@
-"""Cost of the style term's kernels and of a one-GPU texture step whose Gram matrix is too large for `gram`.
+"""Cost of the style term's kernels and of a one-GPU texture step with a large Gram matrix.
 
 1. Kernels (CUDA events over `--launches` launches, 512 x 512, 16 images per rank): the style term as
    PerceptualEngine.style launches it, forward Gram matrices of fakes (NHWC) and targets (NCHW), the MSE and the
    gradient, in the default mode.
-     * gram:        the existing path (`gram` x 2, `gram_mse`, `gram_bwd`) at world 1, R = 48 rows;
-     * rows_w<w>:   the row path (`gram_rows` x 2, `gram_rows_mse`, `gram_rows_bwd`) of ONE rank of w, its 48 rows
-                    against R = 48 w rows of emulated ranks (the gathered batch is already on the device: the
-                    all-gather is not in the number), for w = 1, 2, 4, 8.
+     * rows_w<w>:   `gram_rows` x 2, `gram_rows_mse`, `gram_rows_bwd` of ONE rank of w, its 48 rows against
+                    R = 48 w rows of emulated ranks (the gathered batch is already on the device: the all-gather is
+                    not in the number), for w = 1, 2, 4, 8.
 2. Texture step (`--step-size` x `--step-size`, batch `--step-batch` on one GPU, content and style on with a
-   seeded-random VGG16, graph replay): ms per optimize_parameters().  Batch 48 is 144 Gram rows: the row path.
+   seeded-random VGG16, graph replay): ms per optimize_parameters().  Batch 48 is 144 Gram rows.
 Prints one JSON line with the card's name and power limit.
 
     python tools/bench_style.py [--launches 50] [--steps 10] [--warmup 3]
@@ -49,18 +48,7 @@ def kernel_legs(S: int, per: int, worlds, launches: int) -> dict:
     out = {}
     rl = 3 * per
     acc = torch.zeros(1, dtype=torch.float64, device=dev)
-    fakes = torch.rand(per, S, S, 3, generator=g, device=dev) * 2 - 1
-    targets = torch.rand(per, 3, S, S, generator=g, device=dev) * 4.5 - 2
     dx = torch.zeros(per, S, S, 3, device=dev)
-    go = torch.zeros(rl, rl, dtype=torch.float64, device=dev)
-    gt, m = torch.zeros_like(go), torch.zeros(rl, rl, device=dev)
-
-    def gram_path():
-        ops.gram(fakes, True, go)
-        ops.gram(targets, False, gt)
-        ops.gram_mse(go, gt, 5e-8, acc, m)
-        ops.gram_bwd(m, fakes, True, dx, accumulate=True)
-    out["gram"] = time_launches(gram_path, launches)
     for w in worlds:
         fa = torch.rand(w * per, S, S, 3, generator=g, device=dev) * 2 - 1
         ta = torch.rand(w * per, 3, S, S, generator=g, device=dev) * 4.5 - 2
@@ -105,7 +93,7 @@ def texture_step(B: int, S: int, warmup: int, steps: int) -> dict:
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
     res = {"batch": B, "size": S, "ms_per_step": round(ms, 3), "images_per_s": round(1000.0 * B / ms, 2),
-           "style_rows": m._eng_P.rows, "row_path": m._eng_P.row_path, "graph_replay": len(m._graphs) > 0,
+           "style_rows": m._eng_P.rows, "graph_replay": len(m._graphs) > 0,
            "peak_gb": round(torch.cuda.max_memory_allocated() / 1e9, 2), "G_style": m.get_current_losses()["G_style"]}
     del m, batch
     return res
