@@ -280,7 +280,7 @@ typedef struct sn_norm_act_desc {
   int out_reflect_pad;                   /* 1: planes are [n, h+2, w+2] with ReflectionPad2d(1) */
   float* out_f32; int f32_pitch;         /* optional fp32 copy (residual stream) */
   const float* gamma; const float* beta; /* optional [c] BatchNorm weight / bias: the normalised value is
-                                            gamma * xhat + beta (activation gate included); needs stats, c % 4 == 0 */
+                                            gamma * xhat + beta (activation gate included); needs stats */
 } sn_norm_act_desc;
 int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream);
 
@@ -305,7 +305,8 @@ typedef struct sn_norm_act_bwd_desc {
   double* gstats;                        /* scratch [n][c][2] (needed when stats != NULL) */
   void* dy_hi; void* dy_lo; int dy_pitch, dy_coff; /* split planes of dL/dy */
   int dy_fmt;
-  float* bias_grad;                      /* optional [c], c in {256, 512, 1024}: += sum over pixels of dL/dy (the bias
+  float* bias_grad;                      /* optional [c], c in {256, 512, 1024} ({64, 128, 256} when c % 4 != 0 or a
+                                            row is not 16-byte aligned): += sum over pixels of dL/dy (the bias
                                             gradient of the conv that produced y), fused into the apply pass */
   const float* gamma; const float* beta; /* BatchNorm (both NULL: InstanceNorm / none).  stats hold the (mean, rstd) of
                                             sn_bn_finalize or sn_bn_eval_stats */

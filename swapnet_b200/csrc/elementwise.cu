@@ -55,11 +55,78 @@ __device__ __forceinline__ unsigned long long drop_seed_of(const Args& a) {
   return sn_mix_seed(step_seed, a.stage_id);
 }
 
-__device__ __forceinline__ void store_split(uint16_t* hi, uint16_t* lo, long long off, float v, int fmt) {
-  uint16_t h, l;
-  split16(v, fmt, h, l);
-  hi[off] = h;
-  if (lo) lo[off] = l;
+// V consecutive channels moved as one load or store: V fp32 values (V = 1, 4) or V 16-bit words (V = 1, 4, 8).  The
+// caller guarantees the alignment of the V-wide access.
+template <int V>
+__device__ __forceinline__ void load_f32(const float* p, float v[V]) {
+  static_assert(V == 1 || V == 4, "fp32 vectors are 1 or 4 wide");
+  if constexpr (V == 1) {
+    v[0] = *p;
+  } else {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+  }
+}
+// acc[0..V) += the V fp32 values at p, written out rather than as a loop: the gathers that call it sit inside
+// `unroll 1` loops, where an inner loop costs the backward reduce kernels registers
+template <int V>
+__device__ __forceinline__ void add_f32(const float* p, float acc[V]) {
+  static_assert(V == 1 || V == 4, "fp32 vectors are 1 or 4 wide");
+  if constexpr (V == 1) {
+    acc[0] += *p;
+  } else {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    acc[0] += t.x; acc[1] += t.y; acc[2] += t.z; acc[3] += t.w;
+  }
+}
+template <int V>
+__device__ __forceinline__ void store_f32(float* p, const float v[V]) {
+  static_assert(V == 1 || V == 4, "fp32 vectors are 1 or 4 wide");
+  if constexpr (V == 1) *p = v[0];
+  else *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+}
+// V 16-bit words travel packed, two per 32-bit word: word j sits in bits 16 (j & 1) of u[j / 2]
+template <int V>
+__device__ __forceinline__ void load_w16(const uint16_t* p, uint32_t u[(V + 1) / 2]) {
+  static_assert(V == 1 || V == 4 || V == 8, "16-bit vectors are 1, 4 or 8 wide");
+  if constexpr (V == 1) {
+    u[0] = *p;
+  } else if constexpr (V == 4) {
+    const uint2 t = *reinterpret_cast<const uint2*>(p);
+    u[0] = t.x; u[1] = t.y;
+  } else {
+    const uint4 t = *reinterpret_cast<const uint4*>(p);
+    u[0] = t.x; u[1] = t.y; u[2] = t.z; u[3] = t.w;
+  }
+}
+template <int V>
+__device__ __forceinline__ void store_w16(uint16_t* p, const uint32_t u[(V + 1) / 2]) {
+  static_assert(V == 1 || V == 4 || V == 8, "16-bit vectors are 1, 4 or 8 wide");
+  if constexpr (V == 1) *p = (uint16_t)u[0];
+  else if constexpr (V == 4) *reinterpret_cast<uint2*>(p) = make_uint2(u[0], u[1]);
+  else *reinterpret_cast<uint4*>(p) = make_uint4(u[0], u[1], u[2], u[3]);
+}
+__device__ __forceinline__ uint16_t word16(const uint32_t* u, int j) {
+  return (uint16_t)(u[j >> 1] >> (16 * (j & 1)));
+}
+
+// channel counts are signed ints: C >> log2(V) is one shift where C / V would round towards zero
+__host__ __device__ constexpr int log2_of(int v) { return v > 1 ? 1 + log2_of(v >> 1) : 0; }
+
+// V fp32 values -> split16 words at hi[off..off+V) (and lo, when given)
+template <int V>
+__device__ __forceinline__ void store_split(uint16_t* hi, uint16_t* lo, long long off, const float v[V], int fmt) {
+  uint16_t h[V], l[V];
+#pragma unroll
+  for (int j = 0; j < V; ++j) split16(v[j], fmt, h[j], l[j]);
+  uint32_t ph[(V + 1) / 2], pl[(V + 1) / 2];
+#pragma unroll
+  for (int j = 0; j < (V + 1) / 2; ++j) {
+    ph[j] = (uint32_t)h[2 * j] | (2 * j + 1 < V ? (uint32_t)h[2 * j + 1] << 16 : 0u);
+    pl[j] = (uint32_t)l[2 * j] | (2 * j + 1 < V ? (uint32_t)l[2 * j + 1] << 16 : 0u);
+  }
+  store_w16<V>(hi + off, ph);
+  if (lo) store_w16<V>(lo + off, pl);
 }
 
 // ---------------------------------------------------------------------------------
@@ -96,7 +163,7 @@ __global__ void pack_planes_nchw_kernel(const float* __restrict__ src, int layou
     const int w = i / C, c = i % C;
     if (w0 + w < W) {
       const long long off = (((long long)n * H + h) * W + w0 + w) * pitch + coff + c;
-      store_split(hi, lo, off, tile[c * 33 + w], fmt);
+      store_split<1>(hi, lo, off, &tile[c * 33 + w], fmt);
     }
   }
 }
@@ -108,7 +175,7 @@ __global__ void pack_planes_nhwc_kernel(const float* __restrict__ src, int src_p
        i += (long long)gridDim.x * blockDim.x) {
     const long long pix = i / C;
     const int c = (int)(i - pix * C);
-    store_split(hi, lo, pix * pitch + coff + c, src[pix * src_pitch + c], fmt);
+    store_split<1>(hi, lo, pix * pitch + coff + c, &src[pix * src_pitch + c], fmt);
   }
 }
 
@@ -300,7 +367,8 @@ __global__ void pack_head_weights_kernel(const float* __restrict__ w, int cout, 
     } else {
       off = ((long long)ci * taps_pitch + te) * k_pad + co;  // [ci][taps_pitch >= 25][k_pad]
     }
-    store_split(hi, lo, off, acc * sc, fmt);
+    acc *= sc;
+    store_split<1>(hi, lo, off, &acc, fmt);
   }
 }
 // stacked-phase layout of the same effective taps: dst[row = phase*slot + co][tap9 = (sy+1)*3 + (sx+1)][ci]
@@ -324,7 +392,8 @@ __global__ void pack_head_stacked_kernel(const float* __restrict__ w, int cout, 
       for (int a = 0; a < ny; ++a)
         for (int b = 0; b < nx; ++b) acc += w[(((long long)co * cin + ci) * 4 + kys[a]) * 4 + kxs[b]];
     }
-    store_split(hi, lo, i, acc * sc, fmt);
+    acc *= sc;
+    store_split<1>(hi, lo, i, &acc, fmt);
   }
 }
 __global__ void fold_head_wgrad_kernel(const float* __restrict__ geff, int cout, int cin,
@@ -663,78 +732,48 @@ __global__ void bn_bwd_group_gathered_kernel(double* g, int N, int C, int groups
 }
 
 
-// bias gradient: db[c] = sum over pixels of dy (dy carried as split planes)
-template <bool DET>
-__global__ void bias_grad_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo,
-                                 int pitch, int fmt, long long npix, int C, double* __restrict__ acc,
-                                 double* __restrict__ slots) {
-  __shared__ float s1s[8][33];
-  const int c = blockIdx.x * 32 + threadIdx.x;
-  const long long per = (npix + gridDim.y - 1) / gridDim.y;
-  const long long p0 = blockIdx.y * per;
-  const long long p1 = p0 + per < npix ? p0 + per : npix;
-  double s = 0.0;
-  if (c < C) {
-    float part = 0.f;
-    int cnt = 0;
-    for (long long p = p0 + threadIdx.y; p < p1; p += 8) {
-      float v = decode16(hi[p * pitch + c], fmt);
-      if (lo) v += decode16(lo[p * pitch + c], fmt);
-      part += v;
-      if (++cnt == 64) { s += (double)part; part = 0.f; cnt = 0; }
-    }
-    s += (double)part;
-  }
-  s1s[threadIdx.y][threadIdx.x] = (float)s;  // per-thread partial (<= per/8 terms) fits fp32 well
-  __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
-    double a = 0.0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) a += (double)s1s[j][threadIdx.x];
-    if constexpr (DET) slots[(long long)blockIdx.y * C + c] = a;
-    else atomic_add_f64(&acc[c], a);
-  }
-}
-// 8 channels per thread (one 16-B load per plane); block (G = C/8 groups, 256/G pixel rows)
-template <bool DET>
-__global__ void bias_grad_v8_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo, int pitch,
-                                    int fmt, long long npix, int C, double* __restrict__ acc,
-                                    double* __restrict__ slots) {
-  __shared__ float red[256][8];
+// bias gradient: db[c] = sum over pixels of dy (dy carried as split planes).  V channels per thread (one V-word load
+// per plane); block (bx = min(32, pow2 >= G), 256/bx pixel rows) over the G = ceil(C/V) channel groups
+template <int V, bool DET>
+__global__ void bias_grad_kernel(const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo, int pitch, int fmt,
+                                 long long npix, int C, double* __restrict__ acc, double* __restrict__ slots) {
+  __shared__ float red[256][V];
   const int gch = blockIdx.x * blockDim.x + threadIdx.x;   // channel group
-  const int c = gch * 8;
+  const int c = gch * V;
   const long long per = (npix + gridDim.y - 1) / gridDim.y;
   const long long p0 = blockIdx.y * per;
   const long long p1 = p0 + per < npix ? p0 + per : npix;
-  float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  double d[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  float s[V];
+  double d[V];
+#pragma unroll
+  for (int j = 0; j < V; ++j) {
+    s[j] = 0.f;
+    d[j] = 0.0;
+  }
   if (c < C) {
     int cnt = 0;
     for (long long p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
-      const uint4 vh = *reinterpret_cast<const uint4*>(hi + p * pitch + c);
-      const uint4 vl = lo ? *reinterpret_cast<const uint4*>(lo + p * pitch + c) : make_uint4(0, 0, 0, 0);
-      const uint32_t wh[4] = {vh.x, vh.y, vh.z, vh.w}, wl[4] = {vl.x, vl.y, vl.z, vl.w};
+      uint32_t wh[(V + 1) / 2], wl[(V + 1) / 2];
+      load_w16<V>(hi + p * pitch + c, wh);
+      if (lo) load_w16<V>(lo + p * pitch + c, wl);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        s[2 * j] += decode16((uint16_t)(wh[j] & 0xFFFF), fmt) + (lo ? decode16((uint16_t)(wl[j] & 0xFFFF), fmt) : 0.f);
-        s[2 * j + 1] += decode16((uint16_t)(wh[j] >> 16), fmt) + (lo ? decode16((uint16_t)(wl[j] >> 16), fmt) : 0.f);
-      }
+      for (int j = 0; j < V; ++j) s[j] += decode16(word16(wh, j), fmt) + (lo ? decode16(word16(wl, j), fmt) : 0.f);
       if (++cnt == 64) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { d[j] += (double)s[j]; s[j] = 0.f; }
+        for (int j = 0; j < V; ++j) { d[j] += (double)s[j]; s[j] = 0.f; }
         cnt = 0;
       }
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j) d[j] += (double)s[j];
+    for (int j = 0; j < V; ++j) d[j] += (double)s[j];
   }
   const int slot = threadIdx.y * blockDim.x + threadIdx.x;
 #pragma unroll
-  for (int j = 0; j < 8; ++j) red[slot][j] = (float)d[j];
+  for (int j = 0; j < V; ++j) red[slot][j] = (float)d[j];
   __syncthreads();
   if (threadIdx.y == 0 && c < C) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 0; j < V; ++j) {
       if (c + j >= C) break;
       double u = 0.0;
       for (int r = 0; r < (int)blockDim.y; ++r) u += (double)red[r * blockDim.x + threadIdx.x][j];
@@ -749,8 +788,12 @@ __global__ void bias_grad_finalize_kernel(const double* acc, int C, float* db) {
 }
 
 // ---------------------------------------------------------------------------------
-// InstanceNorm-apply + activation + dropout (+ residual) forward
-// grid (slabs, N); block (cx, py): cx threads over channels, py over pixels
+// InstanceNorm-apply + activation + dropout (+ residual) forward and its backward.
+// V = 4 channels per thread where C % 4 == 0 and the rows are 16-B (fp32) / 8-B (planes) aligned, else V = 1; the host
+// picks the instantiation, the arithmetic per element is the same.  One block = one image n, one slab of pixels and
+// one slice of channels; the slice's per-channel statistics sit in shared memory; threads walk the flattened (pixel,
+// channel group) index so that a warp touches 128 V contiguous bytes.  The kernels are compiled for 4 resident blocks
+// per SM (at most 64 registers): one group in flight per thread, latency hidden by occupancy.
 // ---------------------------------------------------------------------------------
 struct NormActFwdArgs {
   const float* y; int y_pitch;
@@ -766,6 +809,11 @@ struct NormActFwdArgs {
   const float* gamma; const float* beta;   // BatchNorm affine (the AFF kernel instantiations): out = gamma*xhat + beta
 };
 
+// channels of one block's slice: its shared-memory arrays (2 x S floats forward, 4 x S backward apply, two more with
+// the BatchNorm affine) stay within the 48 KB a launch gets without opting in; wider tensors take ceil(C / S) slices
+__host__ __device__ constexpr int fwd_slice(bool aff) { return aff ? 3072 : 4096; }
+constexpr int kApplySlice = 2048;
+
 __device__ __forceinline__ float act_fwd(float v, int act, float slope) {
   if (act == SN_ACT_LRELU) return v > 0.f ? v : v * slope;
   if (act == SN_ACT_RELU) return v > 0.f ? v : 0.f;
@@ -777,104 +825,120 @@ __device__ __forceinline__ float act_grad(float xhat, int act, float slope) {
   return 1.f;
 }
 
-__global__ void norm_act_fwd_kernel(const NormActFwdArgs a) {
+// grid (slabs, N, slices), block 256
+template <int V, bool AFF>
+__global__ void __launch_bounds__(256, 4) norm_act_fwd_kernel(const NormActFwdArgs a) {
+  extern __shared__ float sm[];  // mean[cs], rstd[cs] (+ gamma[cs], beta[cs] when AFF)
+  constexpr int S = fwd_slice(AFF);
+  const int c0 = blockIdx.z * S, cs = min(S, a.C - c0);
+  float* s_mean = sm;
+  float* s_rstd = sm + cs;
+  float* s_gam = sm + 2 * cs;
+  float* s_bet = sm + 3 * cs;
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
   const int n = blockIdx.y;
-  const int HW = a.H * a.W;
+  for (int c = threadIdx.x; c < cs; c += blockDim.x) {
+    s_mean[c] = a.stats ? (float)a.stats[((long long)n * a.C + c0 + c) * 2] : 0.f;
+    s_rstd[c] = a.stats ? (float)a.stats[((long long)n * a.C + c0 + c) * 2 + 1] : 1.f;
+    if constexpr (AFF) {
+      s_gam[c] = a.gamma[c0 + c];
+      s_bet[c] = a.beta[c0 + c];
+    }
+  }
+  __syncthreads();
+  const int HW = a.H * a.W, Q = cs >> log2_of(V);
   const int per = (HW + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    float mean = 0.f, rstd = 1.f;
-    if (a.stats) {
-      mean = (float)a.stats[((long long)n * a.C + c) * 2];
-      rstd = (float)a.stats[((long long)n * a.C + c) * 2 + 1];
-    }
-    for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
-      const long long pix = (long long)n * HW + p;
-      float v = a.y[pix * a.y_pitch + c];
-      v = (v - mean) * rstd;
-      v = act_fwd(v, a.act, a.slope);
+  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
+  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
+    const int pl = i / Q;
+    const int p = p0 + pl;
+    const int cl = (i - pl * Q) * V;   // channel within the slice
+    const int c = c0 + cl;
+    const long long pix = (long long)n * HW + p;
+    float v[V];
+    load_f32<V>(a.y + pix * a.y_pitch + c, v);
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      float t = (v[j] - s_mean[cl + j]) * s_rstd[cl + j];
+      if constexpr (AFF) t = t * s_gam[cl + j] + s_bet[cl + j];
+      t = act_fwd(t, a.act, a.slope);
       if (a.drop_thresh) {
-        const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c, a.drop_thresh);
-        v = keep ? v * a.drop_scale : 0.f;
+        const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
+        t = keep ? t * a.drop_scale : 0.f;
       }
-      if (a.residual) v += a.residual[pix * a.res_pitch + c];
-      if (a.f32) a.f32[pix * a.f32_pitch + c] = v;
-      if (a.hi) {
-        uint16_t h, l, h2 = 0, l2 = 0;
-        split16(v, a.fmt, h, l);
-        if (a.hi2) split16(v, a.fmt2, h2, l2);
-        if (!a.reflect) {
-          const long long off = pix * a.out_pitch + a.out_coff + c;
-          a.hi[off] = h;
-          if (a.lo) a.lo[off] = l;
-          if (a.hi2) {
-            a.hi2[off] = h2;
-            if (a.lo2) a.lo2[off] = l2;
+      v[j] = t;
+    }
+    if (a.residual) {
+      float r[V];
+      load_f32<V>(a.residual + pix * a.res_pitch + c, r);
+#pragma unroll
+      for (int j = 0; j < V; ++j) v[j] += r[j];
+    }
+    if (a.f32) store_f32<V>(a.f32 + pix * a.f32_pitch + c, v);
+    if (a.hi) {
+      if (!a.reflect) {
+        const long long off = pix * a.out_pitch + a.out_coff + c;
+        store_split<V>(a.hi, a.lo, off, v, a.fmt);
+        if (a.hi2) store_split<V>(a.hi2, a.lo2, off, v, a.fmt2);
+      } else {
+        const int hh = p / a.W, ww = p - hh * a.W;
+        const int Hp = a.H + 2, Wp = a.W + 2;
+        const int nr = reflect_pad1_count(hh, a.H), nc = reflect_pad1_count(ww, a.W);
+        for (int ii = 0; ii < nr; ++ii)
+          for (int jj = 0; jj < nc; ++jj) {
+            const long long off = (((long long)n * Hp + reflect_pad1_position(hh, a.H, ii)) * Wp +
+                                   reflect_pad1_position(ww, a.W, jj)) * a.out_pitch + a.out_coff + c;
+            store_split<V>(a.hi, a.lo, off, v, a.fmt);
+            if (a.hi2) store_split<V>(a.hi2, a.lo2, off, v, a.fmt2);
           }
-        } else {
-          const int hh = p / a.W, ww = p - hh * a.W;
-          const int Hp = a.H + 2, Wp = a.W + 2;
-          const int nr = reflect_pad1_count(hh, a.H), nc = reflect_pad1_count(ww, a.W);
-          for (int i = 0; i < nr; ++i)
-            for (int j = 0; j < nc; ++j) {
-              const long long off = (((long long)n * Hp + reflect_pad1_position(hh, a.H, i)) * Wp +
-                                     reflect_pad1_position(ww, a.W, j)) * a.out_pitch + a.out_coff + c;
-              a.hi[off] = h;
-              if (a.lo) a.lo[off] = l;
-              if (a.hi2) {
-                a.hi2[off] = h2;
-                if (a.lo2) a.lo2[off] = l2;
-              }
-            }
-        }
       }
     }
   }
 }
 
-// ---------------------------------------------------------------------------------
-// backward of the same block
-// ---------------------------------------------------------------------------------
 struct GradSrcs {
   sn_grad_src s[SN_MAX_SRC];
   int n;
 };
-// upstream gradient at (n, h, w, c): sum of sources; a reflect-padded source folds its
+// upstream gradient at (n, h, w, c..c+V): sum of sources; a reflect-padded source folds its
 // mirrored border rows/cols back onto the interior pixel (adjoint of ReflectionPad2d(1)).
-__device__ __forceinline__ float gather_one(const sn_grad_src& s, int n, int h, int w, int H, int W, int c) {
-  float acc = 0.f;
-  {
-    if (s.up > 1) {
-      const int u = s.up;
-      for (int a = 0; a < u; ++a)
-        for (int b = 0; b < u; ++b)
-          acc += s.ptr[(((long long)n * H * u + h * u + a) * W * u + w * u + b) * s.pitch + s.c_off + c];
-    } else if (!s.reflect_padded) {
-      acc += s.ptr[(((long long)n * H + h) * W + w) * s.pitch + s.c_off + c];
-    } else {
-      const int Hp = H + 2, Wp = W + 2;
-      const int nr = reflect_pad1_count(h, H), nc = reflect_pad1_count(w, W);
-      // kept as loops: the gathers are inlined once per source, and unrolled blocks of up to 3x3 loads raise the
-      // register count of ce_tanh_bwd and of the backward kernels
+template <int V>
+__device__ __forceinline__ void gather_one(const sn_grad_src& s, int n, int h, int w, int H, int W, int c, float acc[V]) {
+#pragma unroll
+  for (int j = 0; j < V; ++j) acc[j] = 0.f;
+  if (s.up > 1) {
+    const int u = s.up;
+    for (int a = 0; a < u; ++a)
+      for (int b = 0; b < u; ++b)
+        add_f32<V>(s.ptr + (((long long)n * H * u + h * u + a) * W * u + w * u + b) * s.pitch + s.c_off + c, acc);
+  } else if (!s.reflect_padded) {
+    add_f32<V>(s.ptr + (((long long)n * H + h) * W + w) * s.pitch + s.c_off + c, acc);
+  } else {
+    const int Hp = H + 2, Wp = W + 2;
+    const int nr = reflect_pad1_count(h, H), nc = reflect_pad1_count(w, W);
+    // kept as loops: the gathers are inlined once per source, and unrolled blocks of up to 3x3 loads raise the
+    // register count of ce_tanh_bwd and of the backward kernels
 #pragma unroll 1
-      for (int a = 0; a < nr; ++a)
+    for (int a = 0; a < nr; ++a)
 #pragma unroll 1
-        for (int b = 0; b < nc; ++b)
-          acc += s.ptr[(((long long)n * Hp + reflect_pad1_position(h, H, a)) * Wp + reflect_pad1_position(w, W, b)) *
-                           s.pitch + s.c_off + c];
-    }
+      for (int b = 0; b < nc; ++b)
+        add_f32<V>(s.ptr + (((long long)n * Hp + reflect_pad1_position(h, H, a)) * Wp + reflect_pad1_position(w, W, b)) *
+                               s.pitch + s.c_off + c, acc);
   }
-  return acc;
 }
-__device__ __forceinline__ float gather_grad(const GradSrcs& g, int n, int h, int w, int H, int W, int c) {
-  float acc = 0.f;
+template <int V>
+__device__ __forceinline__ void gather_grad(const GradSrcs& g, int n, int h, int w, int H, int W, int c, float acc[V]) {
+  float v[V];
+#pragma unroll
+  for (int j = 0; j < V; ++j) acc[j] = 0.f;
 #pragma unroll
   for (int i = 0; i < SN_MAX_SRC; ++i) {
     if (i >= g.n) break;
-    acc += gather_one(g.s[i], n, h, w, H, W, c);
+    gather_one<V>(g.s[i], n, h, w, H, W, c, v);
+#pragma unroll
+    for (int j = 0; j < V; ++j) acc[j] += v[j];
   }
-  return acc;
 }
 
 struct NormActBwdArgs {
@@ -892,106 +956,196 @@ struct NormActBwdArgs {
   double* slots;      // DET reduce instantiations: per-slab partials of gstats (det_sum_slots)
 };
 
-// gradient w.r.t. xhat (before the InstanceNorm backward), and xhat itself
-__device__ __forceinline__ float grad_xhat(const NormActBwdArgs& a, unsigned long long seed, int n, int p, int c,
-                                           float mean, float rstd, float* xhat_out) {
+// g (w.r.t. the normalised value, gamma*xhat + beta when AFF) and xhat for channels c..c+V
+template <int V, bool AFF>
+__device__ __forceinline__ void grad_xhat(const NormActBwdArgs& a, unsigned long long seed, int n, int p, int c,
+                                          const float* mean, const float* rstd, float g[V], float xh[V],
+                                          const float* gam, const float* bet) {
   const int HW = a.H * a.W;
   const long long pix = (long long)n * HW + p;
   const int h = p / a.W, w = p - h * a.W;
-  const float xhat = (a.y[pix * a.y_pitch + c] - mean) * rstd;
-  float g = 0.f;
+  float yy[V];
+  load_f32<V>(a.y + pix * a.y_pitch + c, yy);
+#pragma unroll
+  for (int j = 0; j < V; ++j) {
+    xh[j] = (yy[j] - mean[j]) * rstd[j];
+    g[j] = 0.f;
+  }
 #pragma unroll
   for (int i = 0; i < SN_MAX_SRC; ++i) {
     if (i >= a.g.n) break;
     const sn_grad_src& s = a.g.s[i];
-    g += gather_one(s, n, h, w, a.H, a.W, c) * act_grad(xhat, s.act >= 0 ? s.act : a.act, a.slope);
+    float gg[V];
+    gather_one<V>(s, n, h, w, a.H, a.W, c, gg);
+    const int act = s.act >= 0 ? s.act : a.act;
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      if constexpr (AFF) g[j] += gg[j] * act_grad(xh[j] * gam[j] + bet[j], act, a.slope);
+      else g[j] += gg[j] * act_grad(xh[j], act, a.slope);
+    }
   }
   if (a.drop_thresh) {
-    const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c, a.drop_thresh);
-    g = keep ? g * a.drop_scale : 0.f;
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
+      g[j] = keep ? g[j] * a.drop_scale : 0.f;
+    }
   }
-  *xhat_out = xhat;
-  return g;
 }
 
-// grid (ceil(C/32), slabs, N), block (32, 8): sums of g and g*xhat per (n, c)
-template <bool DET>
-__global__ void norm_act_bwd_reduce_kernel(const NormActBwdArgs a) {
-  __shared__ float s1s[8][33], s2s[8][33];
+// grid (ceil(Q/bx), slabs, N), block (bx, 256/bx) with Q = C/V channel groups and bx = min(32, pow2 >= Q): thread =
+// channel group, strided over pixels (C = 64 layers, the largest tensors, use bx = 16 and 16 pixel rows at V = 4)
+template <int V, bool AFF, bool DET>
+__global__ void __launch_bounds__(256, 4) norm_act_bwd_reduce_kernel(const NormActBwdArgs a) {
+  __shared__ float red[256][2 * V];
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int c = blockIdx.x * 32 + threadIdx.x;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  const int c = q * V;
   const int n = blockIdx.z;
   const int HW = a.H * a.W;
   const int per = (HW + gridDim.y - 1) / gridDim.y;
   const int p0 = blockIdx.y * per, p1 = min(HW, p0 + per);
-  float s1 = 0.f, s2 = 0.f;
+  float s1[V], s2[V];
+#pragma unroll
+  for (int j = 0; j < V; ++j) s1[j] = 0.f;
+#pragma unroll
+  for (int j = 0; j < V; ++j) s2[j] = 0.f;
   if (c < a.C) {
-    const float mean = (float)a.stats[((long long)n * a.C + c) * 2];
-    const float rstd = (float)a.stats[((long long)n * a.C + c) * 2 + 1];
-    for (int p = p0 + threadIdx.y; p < p1; p += 8) {
-      float xhat;
-      const float g = grad_xhat(a, seed, n, p, c, mean, rstd, &xhat);
-      s1 += g;
-      s2 += g * xhat;
+    float mean[V], rstd[V], gam[V], bet[V];
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      mean[j] = (float)a.stats[((long long)n * a.C + c + j) * 2];
+      rstd[j] = (float)a.stats[((long long)n * a.C + c + j) * 2 + 1];
+      if constexpr (AFF) {
+        gam[j] = a.gamma[c + j];
+        bet[j] = a.beta[c + j];
+      }
+    }
+    for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
+      float g[V], xh[V];
+      grad_xhat<V, AFF>(a, seed, n, p, c, mean, rstd, g, xh, gam, bet);
+#pragma unroll
+      for (int j = 0; j < V; ++j) {
+        s1[j] += g[j];
+        s2[j] += g[j] * xh[j];
+      }
     }
   }
-  s1s[threadIdx.y][threadIdx.x] = s1;
-  s2s[threadIdx.y][threadIdx.x] = s2;
+  const int slot = threadIdx.y * blockDim.x + threadIdx.x;
+#pragma unroll
+  for (int j = 0; j < V; ++j) {
+    red[slot][j] = s1[j];
+    red[slot][V + j] = s2[j];
+  }
   __syncthreads();
   if (threadIdx.y == 0 && c < a.C) {
-    double u = 0.0, v = 0.0;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      u += (double)s1s[j][threadIdx.x];
-      v += (double)s2s[j][threadIdx.x];
-    }
-    const long long i = ((long long)n * a.C + c) * 2;
-    if constexpr (DET) {
-      double* sl = a.slots + (long long)blockIdx.y * (2LL * gridDim.z * a.C);
-      sl[i] = u;
-      sl[i + 1] = v;
-    } else {
-      atomic_add_f64(&a.gstats[i + 0], u);
-      atomic_add_f64(&a.gstats[i + 1], v);
+    for (int j = 0; j < V; ++j) {
+      double u = 0.0, v = 0.0;
+      for (int r = 0; r < (int)blockDim.y; ++r) {
+        u += (double)red[r * blockDim.x + threadIdx.x][j];
+        v += (double)red[r * blockDim.x + threadIdx.x][V + j];
+      }
+      const long long i = ((long long)n * a.C + c + j) * 2;
+      if constexpr (DET) {
+        double* sl = a.slots + (long long)blockIdx.y * (2LL * gridDim.z * a.C);
+        sl[i] = u;
+        sl[i + 1] = v;
+      } else {
+        atomic_add_f64(&a.gstats[i + 0], u);
+        atomic_add_f64(&a.gstats[i + 1], v);
+      }
     }
   }
 }
 
-// grid (slabs, N); block (cx, py)
-__global__ void norm_act_bwd_apply_kernel(const NormActBwdArgs a) {
+// grid (slabs, N, slices), block 256
+template <int V, bool AFF>
+__global__ void __launch_bounds__(256, 4) norm_act_bwd_apply_kernel(const NormActBwdArgs a) {
+  extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x cs (+ gamma, beta when AFF)
+  const int c0 = blockIdx.z * kApplySlice, cs = min(kApplySlice, a.C - c0);
+  float* s_mean = sm;
+  float* s_rstd = sm + cs;
+  float* s_m1 = sm + 2 * cs;
+  float* s_m2 = sm + 3 * cs;
+  float* s_gam = sm + 4 * cs;
+  float* s_bet = sm + 5 * cs;
   const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
   const int n = blockIdx.y;
-  const int HW = a.H * a.W;
+  for (int c = threadIdx.x; c < cs; c += blockDim.x) {
+    const long long k = ((long long)n * a.C + c0 + c) * 2;
+    s_mean[c] = a.stats ? (float)a.stats[k] : 0.f;
+    s_rstd[c] = a.stats ? (float)a.stats[k + 1] : 1.f;
+    s_m1[c] = a.stats ? (float)a.gstats[k] : 0.f;
+    s_m2[c] = a.stats ? (float)a.gstats[k + 1] : 0.f;
+    if constexpr (AFF) {
+      s_gam[c] = a.gamma[c0 + c];
+      s_bet[c] = a.beta[c0 + c];
+    }
+  }
+  __syncthreads();
+  const int HW = a.H * a.W, Q = cs / V;   // a division here: the shift costs the AFF instantiation spills
   const int per = (HW + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    float mean = 0.f, rstd = 1.f, m1 = 0.f, m2 = 0.f;
-    if (a.stats) {
-      mean = (float)a.stats[((long long)n * a.C + c) * 2];
-      rstd = (float)a.stats[((long long)n * a.C + c) * 2 + 1];
-      m1 = (float)a.gstats[((long long)n * a.C + c) * 2];
-      m2 = (float)a.gstats[((long long)n * a.C + c) * 2 + 1];
+  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
+  float bsum[V];   // fused bias gradient: the thread's channel group is fixed when blockDim % Q == 0
+#pragma unroll
+  for (int j = 0; j < V; ++j) bsum[j] = 0.f;
+  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
+    const int pl = i / Q;
+    const int p = p0 + pl;
+    const int cl = (i - pl * Q) * V;   // channel within the slice
+    const int c = c0 + cl;
+    float g[V], xh[V];
+    grad_xhat<V, AFF>(a, seed, n, p, c, s_mean + cl, s_rstd + cl, g, xh, s_gam + cl, s_bet + cl);
+    if constexpr (AFF) {
+#pragma unroll
+      for (int j = 0; j < V; ++j) g[j] = s_gam[cl + j] * s_rstd[cl + j] * (g[j] - s_m1[cl + j] - xh[j] * s_m2[cl + j]);
+    } else if (a.stats) {
+      const float *rstd = s_rstd + cl, *m1 = s_m1 + cl, *m2 = s_m2 + cl;
+#pragma unroll
+      for (int j = 0; j < V; ++j) g[j] = rstd[j] * (g[j] - m1[j] - xh[j] * m2[j]);
     }
-    for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
-      float xhat;
-      float g = grad_xhat(a, seed, n, p, c, mean, rstd, &xhat);
-      if (a.stats) g = rstd * (g - m1 - xhat * m2);
-      const long long off = ((long long)n * HW + p) * a.dy_pitch + a.dy_coff + c;
-      store_split(a.hi, a.lo, off, g, a.fmt);
+    store_split<V>(a.hi, a.lo, ((long long)n * HW + p) * a.dy_pitch + a.dy_coff + c, g, a.fmt);
+#pragma unroll
+    for (int j = 0; j < V; ++j) bsum[j] += g[j];
+  }
+  if (a.bias_grad) {   // host guarantees one slice, blockDim.x % Q == 0 and 4*C >= 256*V floats of scratch
+    __syncthreads();
+    store_f32<V>(sm + threadIdx.x * V, bsum);
+    __syncthreads();
+    if ((int)threadIdx.x < Q) {
+      float t[V], v[V];
+#pragma unroll
+      for (int j = 0; j < V; ++j) t[j] = 0.f;
+      for (int r = threadIdx.x; r < (int)blockDim.x; r += Q) {
+        load_f32<V>(sm + r * V, v);
+#pragma unroll
+        for (int j = 0; j < V; ++j) t[j] += v[j];
+      }
+#pragma unroll
+      for (int j = 0; j < V; ++j) atomicAdd(a.bias_grad + threadIdx.x * V + j, t[j]);
     }
   }
 }
 
+// grid (slabs, N), block 256
+template <int V>
 __global__ void sum_grads_kernel(const GradSrcs g, int H, int W, int C, float* dst, int dst_pitch) {
   const int n = blockIdx.y;
-  const int HW = H * W;
+  const int HW = H * W, Q = C >> log2_of(V);
   const int per = (HW + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  for (int c = threadIdx.x; c < C; c += blockDim.x)
-    for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
-      const int h = p / W, w = p - h * W;
-      dst[((long long)n * HW + p) * dst_pitch + c] = gather_grad(g, n, h, w, H, W, c);
-    }
+  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
+  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
+    const int pl = i / Q;
+    const int p = p0 + pl;
+    const int c = (i - pl * Q) * V;
+    const int h = p / W, w = p - h * W;
+    float v[V];
+    gather_grad<V>(g, n, h, w, H, W, c, v);
+    store_f32<V>(dst + ((long long)n * HW + p) * dst_pitch + c, v);
+  }
 }
 
 // flat (pixel, channel) index: consecutive threads walk consecutive channels then pixels, so the 19-channel
@@ -1009,39 +1163,32 @@ __global__ void tanh_bwd_kernel(const GradSrcs g, const float* __restrict__ out,
     const int p = (int)(pix - (long long)n * HW);
     const int h = p / W, w = p - h * W;
     const float o = out[pix * out_pitch + c];
-    const float v = gather_grad(g, n, h, w, H, W, c) * (1.f - o * o);
-    store_split(hi, lo, pix * dy_pitch + dy_coff + c, v, fmt);
+    float v;
+    gather_grad<1>(g, n, h, w, H, W, c, &v);
+    v *= 1.f - o * o;
+    store_split<1>(hi, lo, pix * dy_pitch + dy_coff + c, &v, fmt);
   }
 }
 
-__global__ void upsample_planes_kernel(const uint16_t* __restrict__ shi, const uint16_t* __restrict__ slo,
-                                       int spitch, int H, int W, int C, int f, uint16_t* __restrict__ dhi,
+// V channels (V 16-bit words) per thread
+template <int V>
+__global__ void upsample_planes_kernel(const uint16_t* __restrict__ shi, const uint16_t* __restrict__ slo, int spitch,
+                                       int H, int W, int CV, int f, uint16_t* __restrict__ dhi,
                                        uint16_t* __restrict__ dlo, int dpitch, long long total) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C);
-    const long long pix = i / C;
+    const int c = (int)(i % CV) * V;
+    const long long pix = i / CV;
     const int w = (int)(pix % W), h = (int)((pix / W) % H);
     const long long n = pix / ((long long)W * H);
     const long long sp = (n * (H / f) + h / f) * (W / f) + w / f;
-    dhi[pix * dpitch + c] = shi[sp * spitch + c];
-    if (dlo) dlo[pix * dpitch + c] = slo[sp * spitch + c];
-  }
-}
-
-// 4 channels (8 bytes) per thread: c, pitches and channel offsets multiples of 4
-__global__ void upsample_planes_v4_kernel(const uint16_t* __restrict__ shi, const uint16_t* __restrict__ slo,
-                                          int spitch, int H, int W, int C4, int f, uint16_t* __restrict__ dhi,
-                                          uint16_t* __restrict__ dlo, int dpitch, long long total) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C4) * 4;
-    const long long pix = i / C4;
-    const int w = (int)(pix % W), h = (int)((pix / W) % H);
-    const long long n = pix / ((long long)W * H);
-    const long long sp = (n * (H / f) + h / f) * (W / f) + w / f;
-    *reinterpret_cast<uint2*>(dhi + pix * dpitch + c) = *reinterpret_cast<const uint2*>(shi + sp * spitch + c);
-    if (dlo) *reinterpret_cast<uint2*>(dlo + pix * dpitch + c) = *reinterpret_cast<const uint2*>(slo + sp * spitch + c);
+    uint32_t t[(V + 1) / 2];
+    load_w16<V>(shi + sp * spitch + c, t);
+    store_w16<V>(dhi + pix * dpitch + c, t);
+    if (dlo) {
+      load_w16<V>(slo + sp * spitch + c, t);
+      store_w16<V>(dlo + pix * dpitch + c, t);
+    }
   }
 }
 
@@ -1261,7 +1408,9 @@ __global__ void __launch_bounds__(128) ce_tanh_bwd_kernel(const float* __restric
         float v = 0.f;
         if (c < C) {
           float gsum = scale * (expf(x[c] - mx) * inv - (c == arg ? 1.f : 0.f));
-          gsum += gather_grad(g, (int)n, h, w, H, W, c);
+          float ge;
+          gather_grad<1>(g, (int)n, h, w, H, W, c, &ge);
+          gsum += ge;
           v = gsum * (1.f - x[c] * x[c]);
         }
         split16(v, fmt, hh[j], ll[j]);
@@ -1399,308 +1548,6 @@ __global__ void tap_gemm_simt_kernel(const SimtArgs a) {
 }
 
 
-// =================================================================================
-// 4-channel vectorised variants (C % 4 == 0, 16-B aligned fp32 rows, 8-B aligned plane rows).
-// One block = one image n and one slab of pixels, all channels; the per-channel statistics sit
-// in shared memory; threads walk the flattened (pixel, channel-quad) index so that a warp
-// touches 512 contiguous bytes.  The norm/activation kernels are compiled for 4 resident blocks
-// per SM (at most 64 registers): one quad in flight per thread, latency hidden by occupancy.
-// =================================================================================
-__device__ __forceinline__ void store_split4(uint16_t* hi, uint16_t* lo, long long off, const float v[4], int fmt) {
-  uint16_t h[4], l[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) split16(v[j], fmt, h[j], l[j]);
-  uint2 ph, pl;
-  ph.x = (uint32_t)h[0] | ((uint32_t)h[1] << 16); ph.y = (uint32_t)h[2] | ((uint32_t)h[3] << 16);
-  pl.x = (uint32_t)l[0] | ((uint32_t)l[1] << 16); pl.y = (uint32_t)l[2] | ((uint32_t)l[3] << 16);
-  *reinterpret_cast<uint2*>(hi + off) = ph;
-  if (lo) *reinterpret_cast<uint2*>(lo + off) = pl;
-}
-
-template <bool AFF>
-__global__ void __launch_bounds__(256, 4) norm_act_fwd_v4_kernel(const NormActFwdArgs a) {
-  extern __shared__ float sm[];  // mean[C], rstd[C] (+ gamma[C], beta[C] when AFF)
-  float* s_mean = sm;
-  float* s_rstd = sm + a.C;
-  float* s_gam = sm + 2 * a.C;
-  float* s_bet = sm + 3 * a.C;
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int n = blockIdx.y;
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    s_mean[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2] : 0.f;
-    s_rstd[c] = a.stats ? (float)a.stats[((long long)n * a.C + c) * 2 + 1] : 1.f;
-    if constexpr (AFF) {
-      s_gam[c] = a.gamma[c];
-      s_bet[c] = a.beta[c];
-    }
-  }
-  __syncthreads();
-  const int HW = a.H * a.W, Q = a.C >> 2;
-  const int per = (HW + gridDim.x - 1) / gridDim.x;
-  const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
-  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
-    const int pl = i / Q;
-    const int p = p0 + pl;
-    const int c = (i - pl * Q) << 2;
-    const long long pix = (long long)n * HW + p;
-    const float4 yv = *reinterpret_cast<const float4*>(a.y + pix * a.y_pitch + c);
-    float v[4] = {yv.x, yv.y, yv.z, yv.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float t = (v[j] - s_mean[c + j]) * s_rstd[c + j];
-      if constexpr (AFF) t = t * s_gam[c + j] + s_bet[c + j];
-      t = act_fwd(t, a.act, a.slope);
-      if (a.drop_thresh) {
-        const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
-        t = keep ? t * a.drop_scale : 0.f;
-      }
-      v[j] = t;
-    }
-    if (a.residual) {
-      const float4 r = *reinterpret_cast<const float4*>(a.residual + pix * a.res_pitch + c);
-      v[0] += r.x; v[1] += r.y; v[2] += r.z; v[3] += r.w;
-    }
-    if (a.f32) *reinterpret_cast<float4*>(a.f32 + pix * a.f32_pitch + c) = make_float4(v[0], v[1], v[2], v[3]);
-    if (a.hi) {
-      if (!a.reflect) {
-        const long long off = pix * a.out_pitch + a.out_coff + c;
-        store_split4(a.hi, a.lo, off, v, a.fmt);
-        if (a.hi2) store_split4(a.hi2, a.lo2, off, v, a.fmt2);
-      } else {
-        const int hh = p / a.W, ww = p - hh * a.W;
-        const int Hp = a.H + 2, Wp = a.W + 2;
-        const int nr = reflect_pad1_count(hh, a.H), nc = reflect_pad1_count(ww, a.W);
-        for (int ii = 0; ii < nr; ++ii)
-          for (int jj = 0; jj < nc; ++jj) {
-            const long long off = (((long long)n * Hp + reflect_pad1_position(hh, a.H, ii)) * Wp +
-                                   reflect_pad1_position(ww, a.W, jj)) * a.out_pitch + a.out_coff + c;
-            store_split4(a.hi, a.lo, off, v, a.fmt);
-            if (a.hi2) store_split4(a.hi2, a.lo2, off, v, a.fmt2);
-          }
-      }
-    }
-  }
-}
-
-__device__ __forceinline__ float4 gather_one4(const sn_grad_src& s, int n, int h, int w, int H, int W, int c) {
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  {
-    if (s.up > 1) {
-      const int u = s.up;
-      for (int a = 0; a < u; ++a)
-        for (int b = 0; b < u; ++b) {
-          const float4 v = *reinterpret_cast<const float4*>(
-              s.ptr + (((long long)n * H * u + h * u + a) * W * u + w * u + b) * s.pitch + s.c_off + c);
-          acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        }
-    } else if (!s.reflect_padded) {
-      const float4 v = *reinterpret_cast<const float4*>(s.ptr + (((long long)n * H + h) * W + w) * s.pitch + s.c_off + c);
-      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-    } else {
-      const int Hp = H + 2, Wp = W + 2;
-      const int nr = reflect_pad1_count(h, H), nc = reflect_pad1_count(w, W);
-#pragma unroll 1
-      for (int a = 0; a < nr; ++a)
-#pragma unroll 1
-        for (int b = 0; b < nc; ++b) {
-          const float4 v = *reinterpret_cast<const float4*>(
-              s.ptr + (((long long)n * Hp + reflect_pad1_position(h, H, a)) * Wp + reflect_pad1_position(w, W, b)) *
-                          s.pitch + s.c_off + c);
-          acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        }
-    }
-  }
-  return acc;
-}
-__device__ __forceinline__ float4 gather_grad4(const GradSrcs& g, int n, int h, int w, int H, int W, int c) {
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int i = 0; i < SN_MAX_SRC; ++i) {
-    if (i >= g.n) break;
-    const float4 v = gather_one4(g.s[i], n, h, w, H, W, c);
-    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-  }
-  return acc;
-}
-
-// g (w.r.t. the normalised value, gamma*xhat + beta when AFF) and xhat for a channel quad
-template <bool AFF = false>
-__device__ __forceinline__ void grad_xhat4(const NormActBwdArgs& a, unsigned long long seed, int n, int p, int c,
-                                           const float* mean, const float* rstd, float g[4], float xh[4],
-                                           const float* gam = nullptr, const float* bet = nullptr) {
-  const int HW = a.H * a.W;
-  const long long pix = (long long)n * HW + p;
-  const int h = p / a.W, w = p - h * a.W;
-  const float4 yv = *reinterpret_cast<const float4*>(a.y + pix * a.y_pitch + c);
-  const float yy[4] = {yv.x, yv.y, yv.z, yv.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    xh[j] = (yy[j] - mean[j]) * rstd[j];
-    g[j] = 0.f;
-  }
-#pragma unroll
-  for (int i = 0; i < SN_MAX_SRC; ++i) {
-    if (i >= a.g.n) break;
-    const sn_grad_src& s = a.g.s[i];
-    const float4 gv = gather_one4(s, n, h, w, a.H, a.W, c);
-    const float gg[4] = {gv.x, gv.y, gv.z, gv.w};
-    const int act = s.act >= 0 ? s.act : a.act;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if constexpr (AFF) g[j] += gg[j] * act_grad(xh[j] * gam[j] + bet[j], act, a.slope);
-      else g[j] += gg[j] * act_grad(xh[j], act, a.slope);
-    }
-  }
-  if (a.drop_thresh) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const bool keep = sn_keep(seed, a.drop_off + (unsigned long long)pix * a.C + c + j, a.drop_thresh);
-      g[j] = keep ? g[j] * a.drop_scale : 0.f;
-    }
-  }
-}
-
-// grid (ceil(Q/bx), slabs, N), block (bx, 256/bx) with bx = min(32, pow2 >= Q): thread = channel quad,
-// strided over pixels (C = 64 layers — the largest tensors — use bx = 16, 16 pixel rows)
-template <bool AFF, bool DET>
-__global__ void __launch_bounds__(256, 4) norm_act_bwd_reduce_v4_kernel(const NormActBwdArgs a) {
-  __shared__ float red[256][8];
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  const int c = q << 2;
-  const int n = blockIdx.z;
-  const int HW = a.H * a.W;
-  const int per = (HW + gridDim.y - 1) / gridDim.y;
-  const int p0 = blockIdx.y * per, p1 = min(HW, p0 + per);
-  float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-  if (c < a.C) {
-    float mean[4], rstd[4], gam[4], bet[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      mean[j] = (float)a.stats[((long long)n * a.C + c + j) * 2];
-      rstd[j] = (float)a.stats[((long long)n * a.C + c + j) * 2 + 1];
-      if constexpr (AFF) {
-        gam[j] = a.gamma[c + j];
-        bet[j] = a.beta[c + j];
-      }
-    }
-    for (int p = p0 + threadIdx.y; p < p1; p += blockDim.y) {
-      float g[4], xh[4];
-      grad_xhat4<AFF>(a, seed, n, p, c, mean, rstd, g, xh, gam, bet);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        s1[j] += g[j];
-        s2[j] += g[j] * xh[j];
-      }
-    }
-  }
-  const int slot = threadIdx.y * blockDim.x + threadIdx.x;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    red[slot][j] = s1[j];
-    red[slot][4 + j] = s2[j];
-  }
-  __syncthreads();
-  if (threadIdx.y == 0 && c < a.C) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      double u = 0.0, v = 0.0;
-      for (int r = 0; r < (int)blockDim.y; ++r) {
-        u += (double)red[r * blockDim.x + threadIdx.x][j];
-        v += (double)red[r * blockDim.x + threadIdx.x][4 + j];
-      }
-      const long long i = ((long long)n * a.C + c + j) * 2;
-      if constexpr (DET) {
-        double* sl = a.slots + (long long)blockIdx.y * (2LL * gridDim.z * a.C);
-        sl[i] = u;
-        sl[i + 1] = v;
-      } else {
-        atomic_add_f64(&a.gstats[i + 0], u);
-        atomic_add_f64(&a.gstats[i + 1], v);
-      }
-    }
-  }
-}
-
-template <bool AFF>
-__global__ void __launch_bounds__(256, 4) norm_act_bwd_apply_v4_kernel(const NormActBwdArgs a) {
-  extern __shared__ float sm[];  // mean, rstd, m1, m2 : 4 x C (+ gamma, beta when AFF)
-  float* s_mean = sm;
-  float* s_rstd = sm + a.C;
-  float* s_m1 = sm + 2 * a.C;
-  float* s_m2 = sm + 3 * a.C;
-  float* s_gam = sm + 4 * a.C;
-  float* s_bet = sm + 5 * a.C;
-  const unsigned long long seed = a.drop_thresh ? drop_seed_of(a) : 0ull;
-  const int n = blockIdx.y;
-  for (int c = threadIdx.x; c < a.C; c += blockDim.x) {
-    const long long k = ((long long)n * a.C + c) * 2;
-    s_mean[c] = a.stats ? (float)a.stats[k] : 0.f;
-    s_rstd[c] = a.stats ? (float)a.stats[k + 1] : 1.f;
-    s_m1[c] = a.stats ? (float)a.gstats[k] : 0.f;
-    s_m2[c] = a.stats ? (float)a.gstats[k + 1] : 0.f;
-    if constexpr (AFF) {
-      s_gam[c] = a.gamma[c];
-      s_bet[c] = a.beta[c];
-    }
-  }
-  __syncthreads();
-  const int HW = a.H * a.W, Q = a.C >> 2;
-  const int per = (HW + gridDim.x - 1) / gridDim.x;
-  const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
-  float bsum[4] = {0.f, 0.f, 0.f, 0.f};   // fused bias gradient: the thread's quad is fixed when blockDim % Q == 0
-  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
-    const int pl = i / Q;
-    const int p = p0 + pl;
-    const int c = (i - pl * Q) << 2;
-    float g[4], xh[4];
-    grad_xhat4<AFF>(a, seed, n, p, c, s_mean + c, s_rstd + c, g, xh, s_gam + c, s_bet + c);
-    if constexpr (AFF) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) g[j] = s_gam[c + j] * s_rstd[c + j] * (g[j] - s_m1[c + j] - xh[j] * s_m2[c + j]);
-    } else if (a.stats) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) g[j] = s_rstd[c + j] * (g[j] - s_m1[c + j] - xh[j] * s_m2[c + j]);
-    }
-    store_split4(a.hi, a.lo, ((long long)n * HW + p) * a.dy_pitch + a.dy_coff + c, g, a.fmt);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) bsum[j] += g[j];
-  }
-  if (a.bias_grad) {   // host guarantees blockDim.x % Q == 0 and 4*C >= 1024 floats of scratch
-    __syncthreads();
-    float4* red = reinterpret_cast<float4*>(sm);
-    red[threadIdx.x] = make_float4(bsum[0], bsum[1], bsum[2], bsum[3]);
-    __syncthreads();
-    if ((int)threadIdx.x < Q) {
-      float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int r = threadIdx.x; r < (int)blockDim.x; r += Q) {
-        const float4 v = red[r];
-        t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
-      }
-      const int c = threadIdx.x << 2;
-      atomicAdd(a.bias_grad + c, t.x); atomicAdd(a.bias_grad + c + 1, t.y);
-      atomicAdd(a.bias_grad + c + 2, t.z); atomicAdd(a.bias_grad + c + 3, t.w);
-    }
-  }
-}
-
-__global__ void sum_grads_v4_kernel(const GradSrcs g, int H, int W, int C, float* dst, int dst_pitch) {
-  const int n = blockIdx.y;
-  const int HW = H * W, Q = C >> 2;
-  const int per = (HW + gridDim.x - 1) / gridDim.x;
-  const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
-  const int i1 = (p1 - p0) * Q;   // slab-relative 32-bit index
-  for (int i = threadIdx.x; i < i1; i += blockDim.x) {
-    const int pl = i / Q;
-    const int p = p0 + pl;
-    const int c = (i - pl * Q) << 2;
-    const int h = p / W, w = p - h * W;
-    *reinterpret_cast<float4*>(dst + ((long long)n * HW + p) * dst_pitch + c) = gather_grad4(g, n, h, w, H, W, c);
-  }
-}
-
 inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 inline bool srcs_vec_ok(const GradSrcs& g) {
   for (int i = 0; i < g.n; ++i)
@@ -1720,20 +1567,6 @@ inline int grid_for(long long total, int threads = kEwThreads) {
   if (g < 1) g = 1;
   return (int)g;
 }
-// block (cx, py) with cx*py == 256, cx = min(pow2 >= C, 256)
-inline dim3 cblock(int C) {
-  int cx = 1;
-  while (cx < C && cx < 256) cx <<= 1;
-  return dim3(cx, 256 / cx, 1);
-}
-inline int slabs_for(int hw, int n, int py) {
-  // enough blocks for ~4 waves, at least `py` pixels each
-  int want = (SN_NUM_SMS * 4 + n - 1) / n;
-  int maxs = (hw + py - 1) / py;
-  if (want > maxs) want = maxs;
-  if (want < 1) want = 1;
-  return want;
-}
 
 }  // namespace
 
@@ -1742,6 +1575,76 @@ inline int slabs_for(int hw, int n, int py) {
     sn_count_launch(1);                        \
     SN_CHECK_CUDA(cudaGetLastError());         \
   } while (0)
+
+// Launchers of the V-templated kernels.  Each entry point computes its vector predicate once and launches the V = 4
+// (bias gradient: 8) or the V = 1 instantiation; both take the same geometry formulas over the C / V channel groups.
+template <int V>
+static int launch_norm_act_fwd(const NormActFwdArgs& a, int n, cudaStream_t st) {
+  const bool aff = a.gamma != nullptr;
+  const int S = fwd_slice(aff), cs = a.C < S ? a.C : S;
+  const dim3 grid(vslabs(a.H * a.W, n), n, (a.C + S - 1) / S);
+  if (aff) norm_act_fwd_kernel<V, true><<<grid, 256, 4 * cs * sizeof(float), st>>>(a);
+  else norm_act_fwd_kernel<V, false><<<grid, 256, 2 * cs * sizeof(float), st>>>(a);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+// ~6 waves of blocks, at least 128 pixels per slab; *nslabs: the slabs (slots per output in deterministic mode)
+template <int V>
+static int launch_norm_act_bwd_reduce(const NormActBwdArgs& a, int n, long long slots_cap, cudaStream_t st,
+                                      int* nslabs) {
+  const int q = a.C / V, hw = a.H * a.W;
+  int bx = 1;
+  while (bx < q && bx < 32) bx <<= 1;
+  const int qg = (q + bx - 1) / bx;
+  int slabs = (SN_NUM_SMS * 6 + n * qg - 1) / (n * qg);
+  if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
+  if (slabs < 1) slabs = 1;
+  *nslabs = slabs;
+  const dim3 grid(qg, slabs, n), blk(bx, 256 / bx);
+  const bool aff = a.gamma != nullptr, det = a.slots != nullptr;
+  if (det) SN_REQUIRE((long long)slabs * 2 * n * a.C <= slots_cap, "norm_act_bwd: det_slots too small");
+  if (aff && det) norm_act_bwd_reduce_kernel<V, true, true><<<grid, blk, 0, st>>>(a);
+  else if (aff) norm_act_bwd_reduce_kernel<V, true, false><<<grid, blk, 0, st>>>(a);
+  else if (det) norm_act_bwd_reduce_kernel<V, false, true><<<grid, blk, 0, st>>>(a);
+  else norm_act_bwd_reduce_kernel<V, false, false><<<grid, blk, 0, st>>>(a);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+template <int V>
+static int launch_norm_act_bwd_apply(const NormActBwdArgs& a, int n, cudaStream_t st) {
+  // the fused bias gradient needs a fixed channel group per thread (256 % (c/V) == 0) and 256 V floats of scratch
+  // (4 c >= 256 V), hence one slice
+  SN_REQUIRE(!a.bias_grad || (256 % (a.C / V) == 0 && 4 * a.C >= 256 * V),
+             "norm_act_bwd: fused bias gradient needs c in {%d, %d, %d} (c=%d)", 64 * V, 128 * V, 256 * V, a.C);
+  const int cs = a.C < kApplySlice ? a.C : kApplySlice;
+  const dim3 grid(vslabs(a.H * a.W, n), n, (a.C + kApplySlice - 1) / kApplySlice);
+  if (a.gamma) norm_act_bwd_apply_kernel<V, true><<<grid, 256, 6 * cs * sizeof(float), st>>>(a);
+  else norm_act_bwd_apply_kernel<V, false><<<grid, 256, 4 * cs * sizeof(float), st>>>(a);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
+
+// block (bx, 256/bx) with bx = min(32, pow2 >= ceil(c/V)); ~6 waves of pixel slabs, at least 256 pixels each
+template <int V>
+static int launch_bias_grad(const uint16_t* hi, const uint16_t* lo, int pitch, int fmt, long long npix, int c,
+                            double* scratch, double* slots, long long slots_cap, cudaStream_t st, int* nslabs) {
+  const int groups = (c + V - 1) / V;
+  int bx = 1;
+  while (bx < groups && bx < 32) bx <<= 1;
+  const int gx = (groups + bx - 1) / bx;
+  long long sl = (SN_NUM_SMS * 6 + gx - 1) / gx;
+  if (sl > (npix + 255) / 256) sl = (npix + 255) / 256;
+  if (sl < 1) sl = 1;
+  *nslabs = (int)sl;
+  SN_REQUIRE(!slots || sl * c <= slots_cap, "bias_grad_det: %lld slots needed, %lld given", sl * c, slots_cap);
+  const dim3 grid(gx, (int)sl), blk(bx, 256 / bx);
+  if (slots) bias_grad_kernel<V, true><<<grid, blk, 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, slots);
+  else bias_grad_kernel<V, false><<<grid, blk, 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, nullptr);
+  LAUNCH_CHECK();
+  return SN_OK;
+}
 
 extern "C" {
 
@@ -1979,24 +1882,8 @@ int sn_norm_act_fwd(const sn_norm_act_desc* d, void* stream) {
                    (!d->out_f32 || (al16(d->out_f32) && d->f32_pitch % 4 == 0)) &&
                    (!d->out_hi || (d->out_pitch % 4 == 0 && d->out_coff % 4 == 0 && ((uintptr_t)d->out_hi & 7) == 0 &&
                                    ((uintptr_t)d->out_lo & 7) == 0 && ((uintptr_t)d->out2_hi & 7) == 0 &&
-                                   ((uintptr_t)d->out2_lo & 7) == 0)) &&
-                   d->c <= 4096;
-  if (d->gamma) {
-    SN_REQUIRE(vec, "norm_act_fwd: the affine (BatchNorm) variant needs c %% 4 == 0 and 16-byte aligned rows (c=%d)", d->c);
-    // mean, rstd, gamma, beta in shared memory: 4 * c floats within the 48 KB a launch gets without opting in
-    SN_REQUIRE(d->c <= 3072, "norm_act_fwd: the affine (BatchNorm) variant supports at most 3072 channels (c=%d)", d->c);
-    dim3 grid(vslabs(d->h * d->w, d->n), d->n);
-    norm_act_fwd_v4_kernel<true><<<grid, 256, 4 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
-  } else if (vec) {
-    dim3 grid(vslabs(d->h * d->w, d->n), d->n);
-    norm_act_fwd_v4_kernel<false><<<grid, 256, 2 * d->c * sizeof(float), (cudaStream_t)stream>>>(a);
-  } else {
-    dim3 blk = cblock(d->c);
-    dim3 grid(slabs_for(d->h * d->w, d->n, blk.y), d->n);
-    norm_act_fwd_kernel<<<grid, blk, 0, (cudaStream_t)stream>>>(a);
-  }
-  LAUNCH_CHECK();
-  return SN_OK;
+                                   ((uintptr_t)d->out2_lo & 7) == 0));
+  return vec ? launch_norm_act_fwd<4>(a, d->n, (cudaStream_t)stream) : launch_norm_act_fwd<1>(a, d->n, (cudaStream_t)stream);
 }
 
 static int fill_srcs(GradSrcs* g, const sn_grad_src* src, int nsrc) {
@@ -2039,8 +1926,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
   const int hw = d->h * d->w;
   const bool vec = (d->c % 4 == 0) && al16(d->y) && (d->y_pitch % 4 == 0) && srcs_vec_ok(a.g) &&
                    (d->dy_pitch % 4 == 0) && (d->dy_coff % 4 == 0) && ((uintptr_t)d->dy_hi & 7) == 0 &&
-                   ((uintptr_t)d->dy_lo & 7) == 0 && d->c <= 2048;
-  SN_REQUIRE(!aff || vec, "norm_act_bwd: the BatchNorm variant needs c %% 4 == 0 and 16-byte aligned rows (c=%d)", d->c);
+                   ((uintptr_t)d->dy_lo & 7) == 0;
   SN_REQUIRE(d->bn_phase >= 0 && d->bn_phase <= 2, "norm_act_bwd: bn_phase %d", d->bn_phase);
   SN_REQUIRE(d->bn_phase == 0 || (aff && d->bn_train), "norm_act_bwd: bn_phase needs the BatchNorm variant in train mode");
   SN_REQUIRE(d->bn_phase != 2 || (d->gstats && d->bn_gathered && d->bn_world >= 1 && d->bn_rank >= 0 && d->bn_rank < d->bn_world),
@@ -2053,31 +1939,9 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
     SN_REQUIRE(d->gstats, "InstanceNorm backward needs gstats scratch");
     SN_CHECK_CUDA(cudaMemsetAsync(d->gstats, 0, sizeof(double) * 2 * d->n * d->c, st));
     int nslabs = 1;
-    if (vec) {
-      int bx = 1;
-      while (bx < d->c / 4 && bx < 32) bx <<= 1;
-      const int qg = (d->c / 4 + bx - 1) / bx;
-      int slabs = (SN_NUM_SMS * 6 + d->n * qg - 1) / (d->n * qg);
-      if (slabs > (hw + 127) / 128) slabs = (hw + 127) / 128;
-      if (slabs < 1) slabs = 1;
-      nslabs = slabs;
-      const dim3 grid(qg, slabs, d->n), blk(bx, 256 / bx);
-      if (det) SN_REQUIRE((long long)slabs * 2 * d->n * d->c <= d->det_slots_cap, "norm_act_bwd: det_slots too small");
-      if (aff && det) norm_act_bwd_reduce_v4_kernel<true, true><<<grid, blk, 0, st>>>(a);
-      else if (aff) norm_act_bwd_reduce_v4_kernel<true, false><<<grid, blk, 0, st>>>(a);
-      else if (det) norm_act_bwd_reduce_v4_kernel<false, true><<<grid, blk, 0, st>>>(a);
-      else norm_act_bwd_reduce_v4_kernel<false, false><<<grid, blk, 0, st>>>(a);
-    } else {
-      const int cg = (d->c + 31) / 32;
-      int slabs = (SN_NUM_SMS * 4 + d->n * cg - 1) / (d->n * cg);
-      if (slabs > (hw + 63) / 64) slabs = (hw + 63) / 64;
-      if (slabs < 1) slabs = 1;
-      nslabs = slabs;
-      if (det) SN_REQUIRE((long long)slabs * 2 * d->n * d->c <= d->det_slots_cap, "norm_act_bwd: det_slots too small");
-      if (det) norm_act_bwd_reduce_kernel<true><<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
-      else norm_act_bwd_reduce_kernel<false><<<dim3(cg, slabs, d->n), dim3(32, 8), 0, st>>>(a);
-    }
-    LAUNCH_CHECK();
+    rc = vec ? launch_norm_act_bwd_reduce<4>(a, d->n, d->det_slots_cap, st, &nslabs)
+             : launch_norm_act_bwd_reduce<1>(a, d->n, d->det_slots_cap, st, &nslabs);
+    if (rc) return rc;
     if (det) {
       SN_CHECK_CUDA(det_sum_slots(d->det_slots, nslabs, 2LL * d->n * d->c, d->gstats, st));
       LAUNCH_CHECK();
@@ -2090,23 +1954,7 @@ int sn_norm_act_bwd(const sn_norm_act_bwd_desc* d, void* stream) {
       gstats_finalize_kernel<<<(d->n * d->c + 255) / 256, 256, 0, st>>>(d->gstats, d->n * d->c, hw);
     LAUNCH_CHECK();
   }
-  if (aff) {
-    dim3 grid(vslabs(hw, d->n), d->n);
-    norm_act_bwd_apply_v4_kernel<true><<<grid, 256, 6 * d->c * sizeof(float), st>>>(a);
-  } else if (vec) {
-    dim3 grid(vslabs(hw, d->n), d->n);
-    // the fused bias gradient needs a fixed quad per thread (256 %% (c/4) == 0) and 256 float4 of scratch (4*c >= 1024)
-    SN_REQUIRE(!d->bias_grad || (256 % (d->c / 4) == 0 && d->c >= 256),
-               "norm_act_bwd: fused bias gradient needs c in {256, 512, 1024} (c=%d)", d->c);
-    norm_act_bwd_apply_v4_kernel<false><<<grid, 256, 4 * d->c * sizeof(float), st>>>(a);
-  } else {
-    SN_REQUIRE(!d->bias_grad, "norm_act_bwd: fused bias gradient is only available on the vectorised path");
-    dim3 blk = cblock(d->c);
-    dim3 grid(slabs_for(hw, d->n, blk.y), d->n);
-    norm_act_bwd_apply_kernel<<<grid, blk, 0, st>>>(a);
-  }
-  LAUNCH_CHECK();
-  return SN_OK;
+  return vec ? launch_norm_act_bwd_apply<4>(a, d->n, st) : launch_norm_act_bwd_apply<1>(a, d->n, st);
 }
 
 
@@ -2114,40 +1962,16 @@ static int bias_grad_impl(const void* dy_hi, const void* dy_lo, int pitch, int c
                           double* scratch, float* db, double* slots, long long slots_cap, cudaStream_t st) {
   SN_REQUIRE(dy_hi && scratch && db, "null pointer");
   SN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * c, st));
-  const int cg = (c + 31) / 32;
-  long long slabs = (SN_NUM_SMS * 4 + cg - 1) / cg;
-  if (slabs > (npix + 63) / 64) slabs = (npix + 63) / 64;
-  if (slabs < 1) slabs = 1;
   const uint16_t* hi = (const uint16_t*)dy_hi + coff;
   const uint16_t* lo = dy_lo ? (const uint16_t*)dy_lo + coff : nullptr;
   const bool v8 = (pitch % 8 == 0) && (coff % 8 == 0) && (((uintptr_t)dy_hi | (uintptr_t)dy_lo) & 15) == 0 &&
                   ((c + 7) / 8 * 8 + coff <= pitch);
-  if (v8) {
-    const int groups = (c + 7) / 8;
-    int bx = 1;
-    while (bx < groups && bx < 32) bx <<= 1;
-    const int gx = (groups + bx - 1) / bx;
-    long long sl = (SN_NUM_SMS * 6 + gx - 1) / gx;
-    if (sl > (npix + 255) / 256) sl = (npix + 255) / 256;
-    if (sl < 1) sl = 1;
-    slabs = sl;
-    SN_REQUIRE(!slots || slabs * c <= slots_cap, "bias_grad_det: %lld slots needed, %lld given", slabs * c, slots_cap);
-    if (slots)
-      bias_grad_v8_kernel<true><<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch,
-                                                                                 slots);
-    else
-      bias_grad_v8_kernel<false><<<dim3(gx, (int)sl), dim3(bx, 256 / bx), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch,
-                                                                                  nullptr);
-  } else {
-    SN_REQUIRE(!slots || slabs * c <= slots_cap, "bias_grad_det: %lld slots needed, %lld given", slabs * c, slots_cap);
-    if (slots)
-      bias_grad_kernel<true><<<dim3(cg, (int)slabs), dim3(32, 8), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, slots);
-    else
-      bias_grad_kernel<false><<<dim3(cg, (int)slabs), dim3(32, 8), 0, st>>>(hi, lo, pitch, fmt, npix, c, scratch, nullptr);
-  }
-  LAUNCH_CHECK();
+  int slabs = 1;
+  const int rc = v8 ? launch_bias_grad<8>(hi, lo, pitch, fmt, npix, c, scratch, slots, slots_cap, st, &slabs)
+                    : launch_bias_grad<1>(hi, lo, pitch, fmt, npix, c, scratch, slots, slots_cap, st, &slabs);
+  if (rc) return rc;
   if (slots) {
-    SN_CHECK_CUDA(det_sum_slots(slots, (int)slabs, (long long)c, scratch, st));
+    SN_CHECK_CUDA(det_sum_slots(slots, slabs, (long long)c, scratch, st));
     LAUNCH_CHECK();
   }
   bias_grad_finalize_kernel<<<(c + 255) / 256, 256, 0, st>>>(scratch, c, db);
@@ -2171,13 +1995,11 @@ int sn_sum_grads(const sn_grad_src* src, int nsrc, int n, int h, int w, int c, f
   GradSrcs g;
   int rc = fill_srcs(&g, src, nsrc);
   if (rc) return rc;
-  if ((c % 4 == 0) && srcs_vec_ok(g) && al16(dst) && (dst_pitch % 4 == 0)) {
-    sum_grads_v4_kernel<<<dim3(vslabs(h * w, n), n), 256, 0, (cudaStream_t)stream>>>(g, h, w, c, dst, dst_pitch);
-  } else {
-    dim3 blk = cblock(c);
-    dim3 grid(slabs_for(h * w, n, blk.y), n);
-    sum_grads_kernel<<<grid, blk, 0, (cudaStream_t)stream>>>(g, h, w, c, dst, dst_pitch);
-  }
+  const dim3 grid(vslabs(h * w, n), n);
+  if ((c % 4 == 0) && srcs_vec_ok(g) && al16(dst) && (dst_pitch % 4 == 0))
+    sum_grads_kernel<4><<<grid, 256, 0, (cudaStream_t)stream>>>(g, h, w, c, dst, dst_pitch);
+  else
+    sum_grads_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(g, h, w, c, dst, dst_pitch);
   LAUNCH_CHECK();
   return SN_OK;
 }
@@ -2198,19 +2020,19 @@ int sn_upsample_planes(const void* src_hi, const void* src_lo, int src_pitch, in
                        int c, int factor, void* dst_hi, void* dst_lo, int dst_pitch, int dst_coff, void* stream) {
   SN_REQUIRE(src_hi && dst_hi && factor >= 1 && h % factor == 0 && w % factor == 0, "bad upsample arguments");
   const long long total = (long long)n * h * w * c;
+  const uint16_t* shi = (const uint16_t*)src_hi + src_coff;
+  const uint16_t* slo = src_lo ? (const uint16_t*)src_lo + src_coff : nullptr;
+  uint16_t* dhi = (uint16_t*)dst_hi + dst_coff;
+  uint16_t* dlo = dst_lo ? (uint16_t*)dst_lo + dst_coff : nullptr;
+  const cudaStream_t st = (cudaStream_t)stream;
   if (c % 4 == 0 && src_pitch % 4 == 0 && dst_pitch % 4 == 0 && src_coff % 4 == 0 && dst_coff % 4 == 0 &&
       ((uintptr_t)src_hi % 8) == 0 && ((uintptr_t)dst_hi % 8) == 0 && (!src_lo || ((uintptr_t)src_lo % 8) == 0) &&
-      (!dst_lo || ((uintptr_t)dst_lo % 8) == 0)) {
-    upsample_planes_v4_kernel<<<grid_for(total / 4), kEwThreads, 0, (cudaStream_t)stream>>>(
-        (const uint16_t*)src_hi + src_coff, src_lo ? (const uint16_t*)src_lo + src_coff : nullptr, src_pitch, h, w,
-        c / 4, factor, (uint16_t*)dst_hi + dst_coff, dst_lo ? (uint16_t*)dst_lo + dst_coff : nullptr, dst_pitch,
-        total / 4);
-    LAUNCH_CHECK();
-    return SN_OK;
-  }
-  upsample_planes_kernel<<<grid_for(total), kEwThreads, 0, (cudaStream_t)stream>>>(
-      (const uint16_t*)src_hi + src_coff, src_lo ? (const uint16_t*)src_lo + src_coff : nullptr, src_pitch, h, w, c,
-      factor, (uint16_t*)dst_hi + dst_coff, dst_lo ? (uint16_t*)dst_lo + dst_coff : nullptr, dst_pitch, total);
+      (!dst_lo || ((uintptr_t)dst_lo % 8) == 0))
+    upsample_planes_kernel<4><<<grid_for(total / 4), kEwThreads, 0, st>>>(shi, slo, src_pitch, h, w, c / 4, factor, dhi,
+                                                                        dlo, dst_pitch, total / 4);
+  else
+    upsample_planes_kernel<1><<<grid_for(total), kEwThreads, 0, st>>>(shi, slo, src_pitch, h, w, c, factor, dhi, dlo,
+                                                                    dst_pitch, total);
   LAUNCH_CHECK();
   return SN_OK;
 }

@@ -628,7 +628,8 @@ def norm_act_fwd(y: torch.Tensor, c: int, stats: Optional[torch.Tensor], act: in
     seed_dev (float32[2] on the device: the 32-bit step seed as its exact 16-bit halves (lo, hi), as
     set_step_params writes them) + stage_id: the per-stage seed is derived on the device from the step seed
     stored there (CUDA-graph replay), drop_seed is then ignored.
-    gamma, beta (fp32 [c]): BatchNorm's affine, applied before the activation."""
+    gamma, beta (fp32 [c]): BatchNorm's affine, applied before the activation.
+    Any c and any row alignment: four channels per thread where c % 4 == 0 and the rows are aligned, else one."""
     n, h, w, _ = y.shape
     pitch = _pitch(y)
     d = SnNormActDesc()
@@ -688,7 +689,9 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
                  bn_rank: int = 0) -> None:
     """ws: deterministic reduction of the normalisation's gradient statistics (then no fused bias_grad).
     bias_grad (fp32 [c], c in {256, 512, 1024}): += per-channel sums of the dy written — the bias gradient of the
-    conv that produced y — inside the apply pass (see fused_bias_grad_ok).
+    conv that produced y — inside the apply pass (see fused_bias_grad_ok; operands that take the one-channel
+    instantiation, c % 4 != 0 or unaligned rows, allow c in {64, 128, 256} instead).
+    Any c and any row alignment: four channels per thread where c % 4 == 0 and the rows are aligned, else one.
     bn = (gamma, beta): BatchNorm backward over `bn_groups` sample groups, with batch (bn_train) or running statistics
     in `stats`; bn_grads = (d gamma, d beta) are accumulated (+=) when given.
     Batch statistics across ranks split the call in two around the gather: bn_phase=1 leaves the per-(n, c)
@@ -727,7 +730,8 @@ def norm_act_bwd(srcs: Sequence[GradSrc], y: torch.Tensor, c: int, stats: Option
 
 
 def fused_bias_grad_ok(c: int) -> bool:
-    """Channel counts for which norm_act_bwd can accumulate the bias gradient itself."""
+    """Channel counts for which norm_act_bwd can accumulate the bias gradient itself, given aligned operands (the
+    engines' are)."""
     return c in (256, 512, 1024)
 
 

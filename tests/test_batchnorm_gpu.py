@@ -27,10 +27,12 @@ def dev():
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("train", [True, False])
 @pytest.mark.parametrize("n,h,c,groups", [(2, 8, 64, 1), (4, 63, 64, 2), (1, 2, 512, 1), (4, 4, 512, 2),
-                                          (2, 63, 256, 2)])
+                                          (2, 63, 256, 2), (2, 8, 19, 1), (2, 3, 3100, 2), (2, 3, 3102, 2)])
 def test_bn_kernels_match_batch_norm(n, h, c, groups, train):
     """sn_plane_sums + sn_bn_finalize (or sn_bn_eval_stats), the affine norm/activation forward and its backward
-    against fp64 F.batch_norm per sample group: output, dL/dy, d gamma, d beta, running buffers, the batch counter."""
+    against fp64 F.batch_norm per sample group: output, dL/dy, d gamma, d beta, running buffers, the batch counter.
+    c = 19 takes the one-channel (V = 1) instantiations; c = 3100 (V = 4) and c = 3102 (V = 1) two channel slices of the
+    forward (3072 per block) and of the apply pass (2048)."""
     from swapnet_b200 import ops
 
     g = torch.Generator().manual_seed(n * 1000 + h * 10 + c + groups)
@@ -51,7 +53,7 @@ def test_bn_kernels_match_batch_norm(n, h, c, groups, train):
         ops.bn_eval_stats(stats, n, c, bn)
     out = torch.zeros(n, h, h, c, device=dev())
     ops.norm_act_fwd(y, c, stats, ops.ACT_LRELU, 0.2, out_f32=out, gamma=bn.weight.data, beta=bn.bias.data)
-    dy = ops.Planes(n, h, h, c, dev(), fmt=ops.FMT_BF16)
+    dy = ops.Planes(n, h, h, (c + 7) // 8 * 8, dev(), c=c, fmt=ops.FMT_BF16)
     gst = torch.zeros(n, c, 2, dtype=torch.float64, device=dev())
     dgam, dbet = torch.zeros(c, device=dev()), torch.zeros(c, device=dev())
     ops.norm_act_bwd([ops.GradSrc(up)], y, c, stats, ops.ACT_LRELU, dy, gst, 0.2, bn=(bn.weight.data, bn.bias.data),

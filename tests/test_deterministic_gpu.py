@@ -373,7 +373,7 @@ def test_reductions_repeat_bit_identically():
     assert relmax(a, _repeat(lambda: ops.plane_stats(y, c, st), st, 1)) < 1e-12
     a = _repeat(lambda: ops.plane_sums(y, c, st, ws=ws), st)
     assert relmax(a, _repeat(lambda: ops.plane_sums(y, c, st), st, 1)) < 1e-12
-    # norm backward reduce (vectorised and scalar paths: c = 64 and c = 19)
+    # norm backward reduce (V = 4 and V = 1 instantiations: c = 64 and c = 19)
     for cc in (64, 19):
         yy = y[..., :cc].contiguous() if cc % 4 == 0 else torch.randn(n, h, w, cc, generator=g).to(dev())
         s2 = torch.zeros(n, cc, 2, dtype=torch.float64, device=dev())
@@ -393,7 +393,7 @@ def test_reductions_repeat_bit_identically():
                     assert all(torch.equal(u, v) for u, v in zip(r, res[0])), f"norm_act_bwd c={cc}"
             outs.append(res[0][0])
         assert relmax(outs[0], outs[1]) < 1e-9
-    # bias gradient: the 8-channel vector kernel (c = 64) and the scalar kernel (odd channel offset)
+    # bias gradient: the V = 8 instantiation (c = 64) and the V = 1 one (odd channel offset)
     dyp, _ = _planes(n, h, w, 64, ops.FMT_BF16, g)
     scratch = torch.zeros(64, dtype=torch.float64, device=dev())
     for view, cc in ((dyp, 64), (dyp.slice(4, 19), 19)):
