@@ -404,7 +404,8 @@ def pack_planes(src, dst: Planes, *, nhwc: bool = False) -> None:
     assert src.dtype == torch.float32
     if nhwc:
         n, h, w, sp = src.shape
-        assert src.stride(3) == 1 and src.stride(2) == sp
+        # dense [n, h, w, sp]: is_contiguous() ignores the strides of size-1 dimensions, which a w = 1 plane may carry
+        assert src.is_contiguous()
         c = dst.c
         for d_ in ((dst,) if dst.twin is None else (dst, dst.twin)):
             check(_lib.load().sn_pack_planes(src.data_ptr(), LAYOUT_NHWC, sp, n, c, h, w, d_.hi_ptr, d_.lo_ptr,

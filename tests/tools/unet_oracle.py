@@ -21,11 +21,11 @@ PIX2PIX_MODES = {"vanilla": "vanilla", "dragan-gp": "vanilla", "dragan-lp": "van
                  "wgan": "wgan", "wgan-gp": "wgan"}
 
 
-def unet_forward(sdG, x, norm: str, train: bool, drop=None):
-    """UnetGenerator(x) with 7 downsamplings -> (output, running buffers after the call, keyed like sdG)."""
+def unet_forward(sdG, x, norm: str, train: bool, drop=None, num_downs: int = NUM_DOWNS):
+    """UnetGenerator(x) with `num_downs` downsamplings -> (output, running buffers after the call, keyed like sdG)."""
     psd = {f"{_P}.{k}": v for k, v in sdG.items()}
     bn = NO.BN(psd, norm, train)
-    out = NO.unet_generator(psd, _P, x, NUM_DOWNS, bn, drop)
+    out = NO.unet_generator(psd, _P, x, num_downs, bn, drop)
     return out, {k[len(_P) + 1:]: v for k, v in bn.bufs.items()}
 
 
